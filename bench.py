@@ -1,7 +1,8 @@
-"""bench.py -- MPC solves/sec of the batched Point2point hot path on B200.
+"""bench.py -- MPC solves/sec of the batched Point2point hot path on an H100.
 
   python bench.py --gpus N --steps K --warmup W          (N>1 under torchrun)
   python bench.py --impl reference ...                   (CPU oracle arm)
+  python bench.py ... --dump-outputs DIR                 (also write the last step's results)
 
 A "step" is one cold solve of the whole batch (BASELINE config 2: batch 1024
 Holonomic Point2point, 10 knot intervals, 3 circular obstacles) from the linear
@@ -9,6 +10,8 @@ initial guess.  `value` times the kernel with inputs resident in HBM (CUDA
 events on the launching stream); `e2e` times the reference-facing C-ABI call
 omg_solve_batch_host with host buffers (H2D + solve + D2H inside).  Per-GPU batch
 is fixed (weak scaling): the batch shards across ranks with no collective.
+The inputs are a pure function of the arguments, so two builds run with the same
+arguments can be compared output for output through --dump-outputs.
 """
 import argparse
 import json
@@ -19,11 +22,14 @@ import time
 
 import numpy as np
 
+# the source tree may be read-only: no bytecode caches written next to the sources
+sys.dont_write_bytecode = True
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
 BATCH = 1024
 L2_FLUSH_BYTES = 256 << 20
+DUMP_LIMIT_BYTES = 64 << 20
 
 
 def parse():
@@ -43,7 +49,10 @@ def parse():
     ap.add_argument('--agents', type=int, default=64, help='config3: agents of the formation')
     ap.add_argument('--formations', type=int, default=1,
                     help='config3: independent formations run side by side in one batch (value counts '
-                         'formation-iterations; 9 x 64 agents fill the 592 resident blocks of one B200)')
+                         'formation-iterations; "limiter" in the output gives the resident blocks per GPU)')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='after the timed steps, write the results of the last timed step as DIR/<name>.npy '
+                         '(float64; rank 0 under torchrun; a fixed, seeded sample of instances above 64 MiB)')
     args = ap.parse_args()
     if args.batch <= 0:
         args.batch = {'config4': 512, 'config4_5obs': 512, 'config5': 256}.get(args.workload, BATCH)
@@ -147,7 +156,26 @@ def measured_peaks():
     if os.path.exists(path):
         d = json.load(open(path))
         return float(d['hbm_gbs']), 'measured'
-    return 6650.0, 'fallback'
+    return 3350.0, 'H100 SXM data sheet (HBM3, 700 W card)'
+
+
+def dump_outputs(path, per_instance, whole=None):
+    """Write every array as path/<name>.npy in float64.  `per_instance` arrays have one row per
+    instance (or agent); when all arrays together exceed DUMP_LIMIT_BYTES, the same fixed, seeded
+    sample of rows is written from each of them, and the sampled row numbers as rows.npy."""
+    os.makedirs(path, exist_ok=True)
+    per_instance = {k: np.asarray(v, dtype=np.float64) for k, v in per_instance.items()}
+    whole = {k: np.asarray(v, dtype=np.float64) for k, v in (whole or {}).items()}
+    total = sum(a.nbytes for a in per_instance.values()) + sum(a.nbytes for a in whole.values())
+    if total > DUMP_LIMIT_BYTES:
+        rows_total = len(next(iter(per_instance.values())))
+        row_bytes = sum(a.nbytes for a in per_instance.values()) / float(rows_total)
+        keep = max(1, int((DUMP_LIMIT_BYTES - sum(a.nbytes for a in whole.values())) // (row_bytes + 8)))
+        rows = np.sort(np.random.default_rng(0).choice(rows_total, min(keep, rows_total), replace=False))
+        per_instance = {k: a[rows] for k, a in per_instance.items()}
+        whole['rows'] = rows.astype(np.float64)
+    for k, a in list(per_instance.items()) + list(whole.items()):
+        np.save(os.path.join(path, k + '.npy'), a)
 
 
 def host_cores():
@@ -202,16 +230,6 @@ WORKLOADS = {
     'config_quadrotor3d_simple': 'SimpleQuadrotor3D Point2point, 2 plate obstacles',
 }
 
-# DRAM traffic of the solver kernel per solve, from the ncu --set full captures
-# (dram__bytes_read.sum + dram__bytes_write.sum of one launch):
-# profiles/r02b_sparse_ncu_raw.txt (config 2, final sparse kernel, 592-solve launch: the writes are L2
-# write-backs of the per-block scratch, 592 blocks x ~190 KB), profiles/r02b_xl_config4_5obs_ncu_raw.txt
-# (config 4 at n = 406, 148-solve launch), profiles/r01_xl_config4_ncu_raw.txt (n = 238, round 1's kernel)
-NCU_DRAM_BYTES_PER_SOLVE = {'config2': (25.132032e6 + 485.795072e6) / 592.,
-                            'config4_5obs': (16.760825e9 + 12.967669e9) / 148.,
-                            'config4': (3.464099e9 + 7.549988e9) / 148.}
-NCU_SOURCE = {'config2': 'profiles/r02b_sparse_ncu_raw.txt', 'config4_5obs': 'profiles/r02b_xl_config4_5obs_ncu_raw.txt',
-              'config4': 'profiles/r01_xl_config4_ncu_raw.txt (round 1 kernel)'}
 # bounded CPU sample: about 20 s of single-core work of the C oracle per measurement
 CPU_SAMPLE = {'config1': 2048, 'config2': 1024, 'config4': 96, 'config4_5obs': 32, 'config5': 512,
               'config_dubins_plain': 256, 'config_holonomic_orient': 32, 'config_quadrotor3d_simple': 256}
@@ -259,6 +277,10 @@ def run_config3(args, rank, world, dev):
         dist.all_reduce(tm, op=dist.ReduceOp.MAX)
     st, it = run.status()
     per = run.formation_residuals()          # collective: every rank
+    if args.dump_outputs and rank == 0:
+        tensors = {k: getattr(run, k).cpu().numpy() for k in ('X', 'z_i', 'l_i', 'z_ij', 'l_ij')}
+        dump_outputs(args.dump_outputs, dict(tensors, status=st, iters=it),
+                     {'residuals': res, 'residuals_per_formation': per})
     if rank == 0:
         ms = float(tm[0])
         tb = pr.tb
@@ -311,6 +333,8 @@ def run_reference(args, rank, world):
         dt = time.perf_counter() - t0
         if k >= args.warmup:
             times.append(dt)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {'x': info['x'], 'status': info['status'], 'iters': info['iters']})
     tot = sum(times)
     value = sample * args.steps / tot
     line = {
@@ -407,6 +431,9 @@ def main():
     kern_ms = tot_ms / args.steps       # one kernel launch per step
     iters = IT.cpu().numpy()
     status = ST.cpu().numpy()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {'x': X.cpu().numpy(), 'lam_g': LAM.cpu().numpy(),
+                                         'f': F.cpu().numpy(), 'status': status, 'iters': iters})
     # ---- e2e: host buffers through the C-ABI call --------------------------------
     pin = lambda a: torch.from_numpy(a).pin_memory().numpy()
     X0p, Pp = pin(X0h), pin(Ph)
@@ -450,10 +477,6 @@ def main():
                       'wave_efficiency': waves / float(np.ceil(waves))},
             'roofline': {'bound': 'hbm', 'achieved': achieved, 'peak': peak,
                          'unit': 'GB/s', 'frac': achieved / peak,
-                         'traffic': (NCU_DRAM_BYTES_PER_SOLVE[args.workload] * B
-                                     if args.workload in NCU_DRAM_BYTES_PER_SOLVE else None),
-                         'traffic_source': ('ncu dram__bytes_read+write per solve of one full launch (%s) x batch'
-                                            % NCU_SOURCE[args.workload]) if args.workload in NCU_SOURCE else None,
                          'peak_source': how,
                          'model': 'staged-KKT bytes/solve = K*2*8*n(n+1)/2 + '
                                   '8(2n+n_par+3m) (SURVEY 8d); K=mean iterations',
@@ -465,9 +488,7 @@ def main():
                                   'peak_tflops': fp64_peak,
                                   'peak_source': 'cuBLAS DGEMM 4096^3 measured in this run',
                                   'note': 'flops the sparse kernel executes (L D L^T gather records x 1.35 '
-                                          'factorisations/iteration + gathers + term streams); the '
-                                          'kernel is bound by instruction issue and dependent latency, '
-                                          'not by this pipe (ncu: profiles/r02b_*)'},
+                                          'factorisations/iteration + gathers + term streams)'},
                          'kernel_ms': kern_ms, 'smem_bytes': info['smem_bytes'],
                          'ctas_per_sm': info['ctas_per_sm']},
             'e2e': {'value': e2e_v, 'unit': 'solves/s',

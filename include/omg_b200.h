@@ -1,5 +1,5 @@
 /* omg_b200.h -- C ABI of libomgb200.so: batched spline-NLP interior-point solve
- * on NVIDIA B200 (sm_100a).
+ * on NVIDIA H100 (sm_90a).
  *
  * This library replaces, for OMG-tools' per-MPC-step solve, the CasADi+IPOPT
  * call of the reference:

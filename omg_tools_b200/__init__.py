@@ -1,4 +1,4 @@
-"""omg_tools_b200: B200-native batched solver for OMG-tools' per-MPC-step
+"""omg_tools_b200: CUDA-native batched solver for OMG-tools' per-MPC-step
 spline-trajectory NLP, behind the reference's Problem.solve()/OptiFather API."""
 from .basics.spline import BSplineBasis, BSpline
 from .basics.shape import (Circle, Polyhedron, Rectangle, Square, Beam,

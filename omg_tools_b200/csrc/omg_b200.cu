@@ -1,5 +1,5 @@
 // omg_b200.cu -- batched primal-dual interior-point solve of OMG-tools' spline
-// NLP on B200 (sm_100a).  One thread block per problem instance (persistent
+// NLP on H100 (sm_90a).  One thread block per problem instance (persistent
 // blocks pull instances from a counter; 2 x 256 threads or 1 x 512 per SM); the
 // per-instance state (KKT envelope, Jacobian values, iterate vectors) lives in
 // shared memory for the duration of the solve, constant tables stream from L2.
@@ -12,8 +12,8 @@
 // problem.py:113, optilayer.py:49-60).  Algorithm = oracle/ipm_ref.py (IPOPT
 // semantics, Waechter & Biegler 2006); tables = basics/lowering.py.
 //
-// Design rules (from tools/ubench/lat.cu on B200: DFMA 8 cyc, LDS 29, SHFL.64 27,
-// rsqrt 62, __syncthreads 28, dependent LDG ~525 cycles):
+// Design rules (a dependent global load costs many times a shared-memory load, a
+// shuffle or a block barrier; tools/ubench/lat.cu measures them on the GPU at hand):
 //   * no dependent chains through global memory: every pass reads one record
 //     per work item (row / column / H position / W slot) and then streams
 //     contiguous 32-byte term records with independent loads;
@@ -2062,10 +2062,8 @@ omg_problem* omg_problem_create(const omg_tables* tb, const omg_options* opt, in
   }
   S.total = off;
   T.hc_nchunk = 0; T.hc_vt = 0;
-  // (experimental, off by default: OMG_B200_HCHUNK=1.  Measured on config 4: the gather phase -21 %
-  //  and the solve -4 % at n = 238 with 16 chunks, nothing at n = 406 where only the panel buffers
-  //  are free (69 chunks); it changes the summation order, which the 300-600-iteration cold starts
-  //  of HolonomicOrient amplify to 3e-4 -- not worth that without a larger gain)
+  // (experimental, off by default: OMG_B200_HCHUNK=1.  It changes the summation order, which the
+  //  300-600-iteration cold starts of HolonomicOrient amplify to 3e-4)
   const char* hce = getenv("OMG_B200_HCHUNK");
   if (ok && hce && atoi(hce) == 1 && h->xl && S.arr[A_JVAL] < 0 && S.arr[A_JSV] < 0 && tb->nnz_h > 0) {
     // chunked J^T Sigma J gather (see the kernel): chunks of whole rows that fit one panel buffer

@@ -79,7 +79,7 @@ class FormationADMMRunner(object):
         """``formations`` > 1 runs that many independent copies of the formation side by side:
         agent a of copy f is global agent f*N + a, its neighbours are offset the same way, so one
         x-update launch, one consensus kernel and one set of collectives advance all copies by one
-        ADMM iteration (64 agents fill a ninth of a B200's resident blocks; nine formations fill it).
+        ADMM iteration (one 64-agent formation leaves most of a GPU's resident blocks idle).
         ``spread`` perturbs copy f's initial guess (relative, seeded by f) so the copies do not
         iterate in lock step.  ``formation_residuals()`` gives the residuals per copy."""
         import torch

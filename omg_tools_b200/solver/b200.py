@@ -329,7 +329,7 @@ def save_tables(tb, path):
 
 
 class B200Solver(object):
-    """Batched interior-point solver on one B200 for one NLP structure."""
+    """Batched interior-point solver on one GPU for one NLP structure."""
 
     def __init__(self, tables, options=None, device=None):
         self.lib = load_library()

@@ -314,7 +314,7 @@ def test_formation_admm_64_agents_matches_oracle(solvers):
     export/tests/formation/test.cpp:200-207).
 
     Tighter where it can be justified: in the first x-update every agent whose interior-point
-    iteration count equals the oracle's agrees to 1e-6 (measured on B200: 1.9e-7 -- summation-order
+    iteration count equals the oracle's agrees to 1e-6 (summation-order
     rounding of the factorisation carried through ~10 Newton steps; 1e-10 in the CPU emulation).  A few of the 64 agents end one iteration
     earlier or later than the oracle (a termination test decided by the last bits, tol = 1e-3,
     problem.py:57): those differ by tol-size (measured 2.7e-4 on agent 24) and their difference

@@ -3,7 +3,7 @@ omg_b200.cu compiled with g++ against a cuda_runtime.h stand-in, every thread of
 fiber, __syncthreads / warp shuffles as barriers.  The emulated kernels -- the same source
 lines the GPU runs -- are compared with the CPU oracle.  This is test infrastructure for a
 container without a GPU: it checks table decoding, the shared-memory layout chosen for a
-B200, barrier placement, the blocked envelope factorisation and the interior-point logic,
+H100, barrier placement, the blocked envelope factorisation and the interior-point logic,
 not performance and not data races.  The product never loads this library."""
 import ctypes as C
 import os
@@ -56,7 +56,7 @@ def test_standard_kernel_matches_oracle(emu, monkeypatch, kernel, name, B, layou
     pr = getattr(sc, name)()
     info = pr.problem.info()
     if layout:
-        assert (info['smem_bytes'], info['ctas_per_sm']) == layout   # the B200 layout
+        assert (info['smem_bytes'], info['ctas_per_sm']) == layout   # the H100 layout
     res, ref = _compare(pr, B, 0.1, 1, 26)
     assert np.array_equal(res['status'], ref['status']) and (ref['status'] == 0).all()
     assert np.array_equal(res['iters'], ref['iters'])
@@ -455,7 +455,7 @@ def test_results_do_not_depend_on_the_thread_schedule(emu, monkeypatch):
     barrier separates from another thread's write would change the result with the order;
     the standard kernel, the XL kernel and its cross / mid-mid Hessian gathers give
     bit-identical solutions and multipliers under every schedule.  (compute-sanitizer
-    racecheck on the GPU, profiles/r01_sanitizer.txt, covers the earlier kernel paths.)"""
+    racecheck on the GPU, tools/sanitize.py, covers the kernel paths on the device.)"""
     cases = []
     for name, B in (('config1', 2), ('config2', 1), ('config_dubins_plain', 1), ('config_bicycle', 1)):
         pr = getattr(sc, name)()

@@ -1,5 +1,5 @@
 """omg_tools_b200/basics/lower_casadi.py: the CasADi-graph -> tables binding that lets the
-REFERENCE's own model reach the B200 solver (INTEGRATION.md, create_nlp branch).
+REFERENCE's own model reach the CUDA solver (INTEGRATION.md, create_nlp branch).
 
 CasADi is not installed here, so the interpreter is driven through the same instruction-level
 interface (n_instructions / instruction_id / instruction_input / instruction_output /

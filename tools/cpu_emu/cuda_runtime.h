@@ -83,7 +83,7 @@ static inline cudaError_t cudaGetDeviceCount(int* n) { *n = 1; return cudaSucces
 static inline cudaError_t cudaSetDevice(int) { return cudaSuccess; }
 static inline cudaError_t cudaGetDevice(int* d) { *d = 0; return cudaSuccess; }
 static inline cudaError_t cudaGetDeviceProperties(cudaDeviceProp* p, int) {
-  // B200 (sm_100a): 227 KB opt-in shared memory per block, 228 KB per SM -- the layout
+  // H100 (sm_90a): 227 KB opt-in shared memory per block, 228 KB per SM -- the layout
   // decisions of omg_problem_create (kernel variant, blocks per SM) are the GPU's
   p->multiProcessorCount = 2; p->sharedMemPerBlockOptin = 232448; p->sharedMemPerMultiprocessor = 233472;
   return cudaSuccess; }

@@ -6,7 +6,7 @@ from omg_tools_b200 import scenarios as sc
 from omg_tools_b200.solver.b200 import B200Solver
 
 nobs = int(sys.argv[1]) if len(sys.argv) > 1 else 2
-B = int(sys.argv[2]) if len(sys.argv) > 2 else 148
+B = int(sys.argv[2]) if len(sys.argv) > 2 else 132   # one block per SM of an H100
 pr = sc.config4(nobs, build_solver=False)
 tb = pr.father.tables
 X0, P = sc.instance_data(pr, 1, jitter=0.0)

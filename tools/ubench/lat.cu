@@ -1,4 +1,4 @@
-// Latency/throughput microbenchmarks for the fp64 path on B200 (single warp / multi warp).
+// Latency/throughput microbenchmarks for the fp64 path (single warp / multi warp).
 #include <cstdio>
 #include <cuda_runtime.h>
 __global__ void k_dfma(double* out, long long* cyc, int n) {
