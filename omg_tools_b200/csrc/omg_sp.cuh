@@ -190,10 +190,19 @@ static inline double sp_rcp(double x) { return 1.0 / x; }
 // out-of-line device code: one copy, outside the instruction range the iterations walk through
 #ifndef OMG_CPU_EMU
 #define SP_COLD __device__ __noinline__
+#define SP_HOT __device__ __noinline__
 #else
 #define SP_COLD static
+#define SP_HOT static inline
 static inline double __dmul_rn(double a, double b) { return a * b; }
 #endif
+
+// IEEE division, log and pow of the per-iteration passes: ONE out-of-line copy each instead of
+// an inlined expansion at every site (tens of call sites, each emitted once per unrolled copy).
+// Correctly rounded division and the libdevice functions give the same bits out of line.
+SP_HOT double sp_div(double a, double b) { return a / b; }
+SP_HOT double sp_log(double x) { return log(x); }
+SP_HOT double sp_pow(double x, double y) { return pow(x, y); }
 
 // objective terms (few, off the hot path): ONE out-of-line copy instead of an unrolled inline
 // expansion at every call site -- the kernel's code is larger than the instruction cache
@@ -649,8 +658,10 @@ __device__ __forceinline__ SpRowDir sp_row_dir(int r, double dsi, double si, dou
   SpRowDir o;
   double sg = 0.0, ph = 0.0;
   o.dzl = 0.0; o.dzu = 0.0;
-  if (r & 1) { const double dl = si - sl; sg += zl / dl; ph -= mu / dl; o.dzl = mu / dl - zl - (zl / dl) * dsi; }
-  if (r & 2) { const double du = su - si; sg += zu / du; ph += mu / du; o.dzu = mu / du - zu + (zu / du) * dsi; }
+  if (r & 1) { const double dl = si - sl, q = sp_div(zl, dl), p = sp_div(mu, dl);
+    sg += q; ph -= p; o.dzl = p - zl - q * dsi; }
+  if (r & 2) { const double du = su - si, q = sp_div(zu, du), p = sp_div(mu, du);
+    sg += q; ph += p; o.dzu = p - zu + q * dsi; }
   o.dy = sg * dsi + ph - yi;
   o.ph = ph;
   return o;
@@ -965,7 +976,7 @@ __device__ __forceinline__ void ipm_body_sp(const DevTab& T, const SpTab& P, con
       // ---- I1: Jacobian values (scaled) + per-row residual terms ---------------------
       // (loads by row type: a bound or multiplier that the row does not have is not fetched)
       SP_STREAM16(P.J, SP_VJ(xe), jval[o_.w & 0xffffu] = acc_;)
-#pragma unroll 2
+#pragma unroll 1
       for (int i = tid; i < m; i += NT) {
         const int r = rt[i];
         const double d = dsc[i];
@@ -977,10 +988,10 @@ __device__ __forceinline__ void ipm_body_sp(const DevTab& T, const SpTab& P, con
         rv[8] += fabs(ci);
         double zl = 0.0, zu = 0.0;
         if (r & 1) { zl = zl_; const double dl = si - sp_bound_lo(lb_, d, rf); const double pz = dl * zl;
-          rv[1] = fmax(rv[1], pz); rv[2] = fmin(rv[2], pz); rv[9] += log(dl); rv[7] += zl; }
+          rv[1] = fmax(rv[1], pz); rv[2] = fmin(rv[2], pz); rv[9] += sp_log(dl); rv[7] += zl; }
         if (r & 2) { zu = zu_; const double du = sp_bound_up(ub_, d, rf) - si; const double pz = du * zu;
-          rv[1] = fmax(rv[1], pz); rv[2] = fmin(rv[2], pz); rv[9] += log(du); rv[7] += zu; }
-        const double gun = gi / d;
+          rv[1] = fmax(rv[1], pz); rv[2] = fmin(rv[2], pz); rv[9] += sp_log(du); rv[7] += zu; }
+        const double gun = sp_div(gi, d);
         if (r & 6) rv[3] = fmax(rv[3], gun - ub_);
         if (r & 5) rv[3] = fmax(rv[3], lb_ - gun);
         if (!(r & 4)) { const double rs = fabs(-yi - zl + zu);
@@ -997,34 +1008,34 @@ __device__ __forceinline__ void ipm_body_sp(const DevTab& T, const SpTab& P, con
       block_reduce<NRED_OPS>(rv, red);
       const double cinf = rv[0], maxprod = rv[1], minprod = rv[2], viol = rv[3];
       const double dinf = fmax(rv[10], rv[4]);
-      const double dinf_un = fmax(rv[10], rv[5]) / ctl.fsc;
+      const double dinf_un = sp_div(fmax(rv[10], rv[5]), ctl.fsc);
       const double ysum = rv[6], zsum = rv[7], theta = rv[8], logsum = rv[9];
-      const double s_d = fmax(S_MAX, (ysum + zsum) / fmax(1.0, (double)(m + n_bounds))) / S_MAX;
-      const double s_c = fmax(S_MAX, zsum / fmax(1.0, (double)n_bounds)) / S_MAX;
+      const double s_d = sp_div(fmax(S_MAX, sp_div(ysum + zsum, fmax(1.0, (double)(m + n_bounds)))), S_MAX);
+      const double s_c = sp_div(fmax(S_MAX, sp_div(zsum, fmax(1.0, (double)n_bounds))), S_MAX);
       double mu = ctl.mu;
       const double cmpl0 = n_bounds ? fmax(fabs(maxprod), fabs(minprod)) : 0.0;
-      const double E0 = fmax(fmax(dinf / s_d, cinf), cmpl0 / s_c);
+      const double E0 = fmax(fmax(sp_div(dinf, s_d), cinf), sp_div(cmpl0, s_c));
       TICK(2);
       // ---- I3: termination + barrier update (uniform) -----------------------------------
       int status = -1;
       if (!isfinite(E0) || !isfinite(theta)) status = OMG_INVALID_NUMBER_DETECTED;
       else if (E0 <= O.tol && dinf_un <= O.dual_inf_tol && viol <= O.constr_viol_tol &&
-               cmpl0 / ctl.fsc <= O.compl_inf_tol) status = OMG_SOLVE_SUCCEEDED;
+               sp_div(cmpl0, ctl.fsc) <= O.compl_inf_tol) status = OMG_SOLVE_SUCCEEDED;
       else if (iter >= O.max_iter) status = OMG_MAX_ITER_EXCEEDED;
       if (tracing && tid == 0 && iter < TRACE_ROWS - 2) {
         double* tr = A.trace + iter * TRACE_COLS;
-        tr[0] = iter; tr[1] = ctl.f / ctl.fsc; tr[2] = cinf; tr[3] = dinf; tr[4] = mu; tr[5] = E0;
+        tr[0] = iter; tr[1] = sp_div(ctl.f, ctl.fsc); tr[2] = cinf; tr[3] = dinf; tr[4] = mu; tr[5] = E0;
         tr[6] = ctl.alpha; tr[7] = ctl.delta_w;
       }
       if (status >= 0) { if (tid == 0) { ctl.status = status; ctl.iter = iter; } break; }
       {
-        const double mu_min = fmin(O.tol, O.compl_inf_tol * ctl.fsc) / (KAPPA_EPS + 1.0);
+        const double mu_min = sp_div(fmin(O.tol, O.compl_inf_tol * ctl.fsc), KAPPA_EPS + 1.0);
         bool changed = false;
         for (;;) {
           const double cm = n_bounds ? fmax(fabs(maxprod - mu), fabs(minprod - mu)) : 0.0;
-          const double Emu = fmax(fmax(dinf / s_d, cinf), cm / s_c);
+          const double Emu = fmax(fmax(sp_div(dinf, s_d), cinf), sp_div(cm, s_c));
           if (Emu <= KAPPA_EPS * mu && mu > mu_min) {
-            mu = fmax(mu_min, fmin(KAPPA_MU * mu, pow(mu, THETA_MU)));
+            mu = fmax(mu_min, fmin(KAPPA_MU * mu, sp_pow(mu, THETA_MU)));
             changed = true;
           } else break;
         }
@@ -1045,7 +1056,7 @@ __device__ __forceinline__ void ipm_body_sp(const DevTab& T, const SpTab& P, con
       const double tau = ctl.tau;
       TICK(3);
       // ---- I4: Sigma, w = Sigma r_d + phi_s ----------------------------------------------
-#pragma unroll 2
+#pragma unroll 1
       for (int i = tid; i < m; i += NT) {
         const int r = rt[i];
         double sg = 0.0, ph = 0.0, rdd = 0.0;
@@ -1053,8 +1064,8 @@ __device__ __forceinline__ void ipm_body_sp(const DevTab& T, const SpTab& P, con
         if (!(r & 4)) {
           const double si = s[i];
           rdd = g[i] - si;
-          if (r & 1) { const double dl = si - sp_bound_lo(lbg[i], d, rf); sg += zL[i] / dl; ph -= mu / dl; }
-          if (r & 2) { const double du = sp_bound_up(ubg[i], d, rf) - si; sg += zU[i] / du; ph += mu / du; }
+          if (r & 1) { const double dl = si - sp_bound_lo(lbg[i], d, rf); sg += sp_div(zL[i], dl); ph -= sp_div(mu, dl); }
+          if (r & 2) { const double du = sp_bound_up(ubg[i], d, rf) - si; sg += sp_div(zU[i], du); ph += sp_div(mu, du); }
         }
         sg2[i] = sg * d * d;
         wv[i] = d * ((r & 4) ? y[i] : (sg * rdd + ph));
@@ -1113,7 +1124,7 @@ __device__ __forceinline__ void ipm_body_sp(const DevTab& T, const SpTab& P, con
         TICK(7);
         if (!ctl.fail) break;
         if (tid == 0) {
-          if (ctl.eq_fail) ctl.delta_c = DELTA_C_VAL * pow(mu, DELTA_C_EXP);
+          if (ctl.eq_fail) ctl.delta_c = DELTA_C_VAL * sp_pow(mu, DELTA_C_EXP);
           if (ctl.first_try) {
             ctl.delta_w = (ctl.delta_w_last == 0.0) ? DELTA_W0
                           : fmax(DELTA_W_MIN, KAPPA_W_MINUS * ctl.delta_w_last);
@@ -1146,7 +1157,7 @@ __device__ __forceinline__ void ipm_body_sp(const DevTab& T, const SpTab& P, con
       //  record: a = x0, b = column, c = row)
       SP_STREAM16(P.R, SP_COEF(o_) * V[o_.z & 0x7fffu] * xe[o_.z >> 16] * dx[o_.w & 0xffffu], ds[o_.w >> 16] = acc_;)
       __syncthreads();
-#pragma unroll 2
+#pragma unroll 1
       for (int i = tid; i < m; i += NT) {
         const int r = rt[i];
         if (r & 4) { ds[i] = 0.0; continue; }
@@ -1158,11 +1169,11 @@ __device__ __forceinline__ void ipm_body_sp(const DevTab& T, const SpTab& P, con
         const double sl = (r & 1) ? sp_bound_lo(lbg[i], d, rf) : 0.0, su = (r & 2) ? sp_bound_up(ubg[i], d, rf) : 0.0;
         const SpRowDir dr = sp_row_dir(r, dsi, si, zl, zu, sl, su, y[i], mu);
         if (r & 1) { const double dl = si - sl;
-          if (dsi < 0.0) sv[0] = fmin(sv[0], -tau * dl / dsi);
-          if (dr.dzl < 0.0) sv[1] = fmin(sv[1], -tau * zl / dr.dzl); }
+          if (dsi < 0.0) sv[0] = fmin(sv[0], sp_div(-tau * dl, dsi));
+          if (dr.dzl < 0.0) sv[1] = fmin(sv[1], sp_div(-tau * zl, dr.dzl)); }
         if (r & 2) { const double du = su - si;
-          if (dsi > 0.0) sv[0] = fmin(sv[0], tau * du / dsi);
-          if (dr.dzu < 0.0) sv[1] = fmin(sv[1], -tau * zu / dr.dzu); }
+          if (dsi > 0.0) sv[0] = fmin(sv[0], sp_div(tau * du, dsi));
+          if (dr.dzu < 0.0) sv[1] = fmin(sv[1], sp_div(-tau * zu, dr.dzu)); }
         ds[i] = dsi;
         sv[2] += dr.ph * dsi;
       }
@@ -1174,9 +1185,9 @@ __device__ __forceinline__ void ipm_body_sp(const DevTab& T, const SpTab& P, con
       const double theta0 = ctl.theta, phi0 = ctl.phi;
       double a_min;
       if (gphi < 0.0) {
-        a_min = fmin(GAMMA_THETA, GAMMA_PHI * theta0 / (-gphi));
+        a_min = fmin(GAMMA_THETA, sp_div(GAMMA_PHI * theta0, -gphi));
         if (theta0 <= ctl.theta_min)
-          a_min = fmin(a_min, DELTA_LS * pow(theta0, S_THETA) / pow(-gphi, S_PHI));
+          a_min = fmin(a_min, sp_div(DELTA_LS * sp_pow(theta0, S_THETA), sp_pow(-gphi, S_PHI)));
       } else a_min = GAMMA_THETA;
       a_min *= GAMMA_ALPHA;
       double alpha = a_p;
@@ -1192,7 +1203,7 @@ __device__ __forceinline__ void ipm_body_sp(const DevTab& T, const SpTab& P, con
         __syncthreads();
         double tv[3];
         tv[0] = 0.0; tv[1] = 0.0; tv[2] = 0.0;
-#pragma unroll 2
+#pragma unroll 1
         for (int i = tid; i < m; i += NT) {
           const int r = rt[i];
           const double d = dsc[i];
@@ -1202,8 +1213,8 @@ __device__ __forceinline__ void ipm_body_sp(const DevTab& T, const SpTab& P, con
           else {
             const double si = s[i] + alpha * ds[i];
             tv[0] += fabs(gi - si);
-            if (r & 1) tv[1] += log(si - sp_bound_lo(lbg[i], d, rf));
-            if (r & 2) tv[1] += log(sp_bound_up(ubg[i], d, rf) - si);
+            if (r & 1) tv[1] += sp_log(si - sp_bound_lo(lbg[i], d, rf));
+            if (r & 2) tv[1] += sp_log(sp_bound_up(ubg[i], d, rf) - si);
           }
         }
         for (int t = tid; t < T.n_f; t += NT) tv[2] += sp_eval_range(T.Ft, t, t + 1, V, xt);
@@ -1219,7 +1230,7 @@ __device__ __forceinline__ void ipm_body_sp(const DevTab& T, const SpTab& P, con
         ftype = false;
         if (ok) {
           const bool switching = (theta0 <= ctl.theta_min && gphi < 0.0 &&
-                                  alpha * pow(-gphi, S_PHI) > DELTA_LS * pow(theta0, S_THETA));
+                                  alpha * sp_pow(-gphi, S_PHI) > DELTA_LS * sp_pow(theta0, S_THETA));
           if (switching) { ok = cmp_le(pht - phi0, ETA_PHI * alpha * gphi, phi0); ftype = ok; }
           else ok = cmp_le(tht, (1.0 - GAMMA_THETA) * theta0, theta0) ||
                     cmp_le(pht - phi0, -GAMMA_PHI * theta0, phi0);
@@ -1262,7 +1273,7 @@ __device__ __forceinline__ void ipm_body_sp(const DevTab& T, const SpTab& P, con
       TICK(12);
       // ---- I12: accept: the step of the pass I10 evaluated again (s, z, y, mu unchanged) ----
       for (int j = tid; j <= n; j += NT) xe[j] = (j < n) ? xt[j] : 1.0;
-#pragma unroll 2
+#pragma unroll 1
       for (int i = tid; i < m; i += NT) {
         const int r = rt[i];
         const double d = dsc[i], yi = y[i];
@@ -1278,9 +1289,9 @@ __device__ __forceinline__ void ipm_body_sp(const DevTab& T, const SpTab& P, con
           const double si = s0 + alpha * dsi;
           s[i] = si;
           if (r & 1) { const double dl = si - sl; double z = zl + a_d * dr.dzl;
-            z = fmin(fmax(z, mu / (KAPPA_SIGMA * dl)), KAPPA_SIGMA * mu / dl); zL[i] = z; }
+            z = fmin(fmax(z, sp_div(mu, KAPPA_SIGMA * dl)), sp_div(KAPPA_SIGMA * mu, dl)); zL[i] = z; }
           if (r & 2) { const double du = su - si; double z = zu + a_d * dr.dzu;
-            z = fmin(fmax(z, mu / (KAPPA_SIGMA * du)), KAPPA_SIGMA * mu / du); zU[i] = z; }
+            z = fmin(fmax(z, sp_div(mu, KAPPA_SIGMA * du)), sp_div(KAPPA_SIGMA * mu, du)); zU[i] = z; }
         }
       }
       __syncthreads();
