@@ -17,6 +17,7 @@ struct SpSym {
   std::vector<std::vector<int>> st_true;      // struct without the explicit zeros of the supernode padding
   std::vector<int> sn_first, sn_w;            // first column / width of the supernode of a column (root: itself, 1)
   int n_pad = 0;                              // explicit zeros stored
+  int max_sn_pad = 0;                         // ... by the supernode with the most
   int idx(int i, int j) const {               // L index of entry (row i, column j); i == N: rhs
     if (j >= R0) return colptr[j] + (i - j);
     if (i == j) return colptr[j];
@@ -122,6 +123,7 @@ static bool sp_symbolic(const omg_tables* tb, SpSym& Y, std::string* why) {
       path.push_back(p); sn_id[p] = id;
       total_z += newz - zcur; zcur = newz;
     }
+    Y.max_sn_pad = std::max(Y.max_sn_pad, zcur);
     paths.push_back(path);
   }
   Y.n_pad = total_z;
@@ -230,6 +232,11 @@ static bool sp_setup(omg_problem* h, const omg_tables* tb, const cudaDeviceProp&
   SpTab& P = h->P;
   memset(&P, 0, sizeof(P));
   bool ok = true;
+  // counters of the structure line: which branches of sp_factor / sp_back_solve this structure
+  // runs, and how close it comes to the packing limits (tests/test_sparse_structures.py)
+  int eq_lev = 0, eq_panel = 0, eq_root = 0, n_snw[SP_SNW + 1] = {0}, max_col = 0, max_gather = 0,
+      max_slices = 0, max_blk = 0, max_prounds = 0, max_nq = 0, max_brounds = 0;
+  for (int j = 0; j < R0; ++j) max_col = std::max(max_col, Y.len[j]);
   P.nt = nt;
   P.zslot = Y.Lsize; P.Lsz = (Y.Lsize + 2) & ~1;
   P.R0 = R0; P.nr = nr; P.n_lev = Y.n_lev; P.root0 = Y.colptr[R0];
@@ -264,6 +271,7 @@ static bool sp_setup(omg_problem* h, const omg_tables* tb, const cudaDeviceProp&
   for (int c0 = 0; c0 < R0; ++c0) {
     if (Y.sn_first[c0] != c0) continue;
     const int w = Y.sn_w[c0];
+    n_snw[w]++;
     const unsigned snoff = (unsigned)sntab.size() * 16u;
     unsigned dl[4] = {0u, 0u, 0u, 0u}, rr[4];
     for (int t = 0; t < 4; ++t) {
@@ -284,6 +292,7 @@ static bool sp_setup(omg_problem* h, const omg_tables* tb, const cudaDeviceProp&
       }
     }
   }
+  for (const std::vector<uint2>& pl : plist) max_gather = std::max(max_gather, (int)pl.size());
   const unsigned sn_dummy = (unsigned)sntab.size() * 16u;           // pad records: 0 * rd[N] * 0
   sntab.push_back(make_uint4(0u, ((unsigned)N * 8u) << 16, ((unsigned)N * 8u) | (((unsigned)N * 8u) << 16), (unsigned)N * 8u));
   if (sntab.size() * 16u >= 65536u) { *why = "too many supernodes"; return false; }
@@ -302,6 +311,7 @@ static bool sp_setup(omg_problem* h, const omg_tables* tb, const cudaDeviceProp&
         for (int e = Y.colptr[j]; e < Y.colptr[j + 1]; ++e) {
           lidx.push_back(e);
           const bool piv = (e == Y.colptr[j]) && Y.sn_w[j] == 1;    // wider supernodes: pivots in the panel step
+          if (piv && is_eq_pos[j]) ++eq_lev;
           ents.push_back((unsigned)e | ((unsigned)j << 13) | (piv ? (1u << 24) : 0u) |
                          ((piv && is_eq_pos[j]) ? (1u << 25) : 0u));
         }
@@ -311,6 +321,7 @@ static bool sp_setup(omg_problem* h, const omg_tables* tb, const cudaDeviceProp&
     std::vector<int> ord(ents.size());
     for (size_t q = 0; q < ord.size(); ++q) ord[q] = (int)q;
     std::stable_sort(ord.begin(), ord.end(), [&](int a, int b) { return plist[lidx[a]].size() > plist[lidx[b]].size(); });
+    max_slices = std::max(max_slices, (int)((ord.size() + 31) / 32));
     lev_ptr.push_back((int)(fdesc.size() / 32));
     for (size_t q0 = 0; q0 < ord.size(); q0 += 32) {
       size_t mx = 0;
@@ -345,13 +356,14 @@ static bool sp_setup(omg_problem* h, const omg_tables* tb, const cudaDeviceProp&
         if (Y.lev[c0] != lv || Y.sn_first[c0] != c0 || Y.sn_w[c0] < 2) continue;
         const int w = Y.sn_w[c0];
         unsigned eqb = 0, cb[4] = {0u, 0u, 0u, 0u};
-        for (int t = 0; t < w; ++t) { cb[t] = (unsigned)Y.colptr[c0 + t] * 8u; if (is_eq_pos[c0 + t]) eqb |= 1u << t; }
+        for (int t = 0; t < w; ++t) { cb[t] = (unsigned)Y.colptr[c0 + t] * 8u; if (is_eq_pos[c0 + t]) { eqb |= 1u << t; ++eq_panel; } }
         const int nR = Y.len[c0 + w - 1];                     // rows below the block (+ the rhs row)
         const unsigned head = (unsigned)c0 | ((unsigned)w << 11) | (eqb << 17) | 0x80000000u;
         for (int r = 0; r <= nR; ++r) rows.push_back(make_uint4(head, cb[0] | (cb[1] << 16), cb[2] | (cb[3] << 16), (unsigned)r));
         for (int q = 1; q < w; ++q) blk.push_back(make_uint4(head | ((unsigned)q << 14), cb[0] | (cb[1] << 16), cb[2] | (cb[3] << 16), 0u));
       }
       if ((int)blk.size() > nt) { *why = "too many supernodes on one level"; return false; }
+      max_blk = std::max(max_blk, (int)blk.size());
       if (!rows.empty() || !blk.empty()) {
         const size_t tot = rows.size() + blk.size();
         const size_t padded = (tot + nt - 1) / nt * nt;
@@ -361,6 +373,7 @@ static bool sp_setup(omg_problem* h, const omg_tables* tb, const cudaDeviceProp&
         // (rows that would share the last round with the block rows stay where they are: a
         //  thread has at most one task per round)
         if (rows.size() > padded - blk.size()) { *why = "panel round overflow"; return false; }
+        max_prounds = std::max(max_prounds, (int)(padded / nt));
         tasks.insert(tasks.end(), lvl.begin(), lvl.end());
       }
     }
@@ -377,6 +390,7 @@ static bool sp_setup(omg_problem* h, const omg_tables* tb, const cudaDeviceProp&
       for (int k0 = 0; k0 <= kmax; k0 += SP_RCW) {
         const int cnt = std::min(SP_RCW, kmax - k0 + 1);
         const bool has_diag = (i < nr && k0 <= i && i < k0 + cnt);
+        if (has_diag && is_eq_pos[R0 + i]) ++eq_root;
         chunks.push_back((unsigned)i | ((unsigned)k0 << 6) | ((unsigned)cnt << 12) |
                          ((has_diag && is_eq_pos[R0 + i]) ? 0x10000u : 0u));
       }
@@ -416,6 +430,8 @@ static bool sp_setup(omg_problem* h, const omg_tables* tb, const cudaDeviceProp&
         maxlen = std::max(maxlen, cntj);
       }
       const unsigned nq = (unsigned)std::max(1, (maxlen + 7) / 8);
+      max_nq = std::max(max_nq, (int)nq);
+      max_brounds = std::max(max_brounds, (int)((bins.size() + wpr - 1) / wpr));
       for (size_t b0 = 0; b0 < bins.size(); b0 += wpr) {
         for (int t = 0; t < nt; ++t) {
           const size_t b = b0 + (size_t)(t >> 5);
@@ -634,5 +650,13 @@ static bool sp_setup(omg_problem* h, const omg_tables* tb, const cudaDeviceProp&
                " pairs=" + std::to_string(fpair.size() * 2) + " nt=" + std::to_string(nt) +
                " ctas/SM=" + std::to_string(occ) + " smem=" + std::to_string(h->sp_smem_bytes) +
                " scratch/iter=" + std::to_string(touched);
+  auto kv = [&](const char* k, int v) { h->sp_info += std::string(" ") + k + "=" + std::to_string(v); };
+  h->sp_info += " |";
+  kv("eqpiv-level", eq_lev); kv("eqpiv-panel", eq_panel); kv("eqpiv-root", eq_root);
+  for (int w = 1; w <= SP_SNW; ++w) kv(("sn" + std::to_string(w)).c_str(), n_snw[w]);
+  kv("zeros", Y.n_pad); kv("max-sn-zeros", Y.max_sn_pad); kv("max-col", max_col);
+  kv("max-gather", max_gather); kv("max-nq", max_nq); kv("max-slices", max_slices);
+  kv("max-block-rows", max_blk); kv("max-panel-rounds", max_prounds); kv("max-back-rounds", max_brounds);
+  kv("root-mod4", nr % 4);
   return true;
 }
