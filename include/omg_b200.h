@@ -260,6 +260,33 @@ int omg_integrate_rk4(int32_t model, int32_t B, int32_t n_state, int32_t n_input
                       const double* state0, const double* inputs, double sample_time,
                       int32_t steps, double* stateT, void* stream);
 
+/* Closed-loop plant step of a batch after the solve of MPC step `step` (reference
+ * Vehicle.simulate / predict with ideal_update = ideal_prediction = False, vehicle.py:302-337,
+ * 359-449).  DEVICE: x [B x n] spline coefficients (column c of the input splines at c*L),
+ * plant_x [B x n_state], plant_u [B x n_input] (plant state and last applied input at t_k),
+ * outputs plant_x_next, plant_u_next (at t_k + n_samp*sample_time; may alias plant_x,
+ * plant_u), pred_x, pred_u, and scratch [B x n_input x (n_traj + 24)] (disturb only).
+ * HOST: R0, R1 [(n_samp+1) x L] basis and derivative rows (derivative divided by the horizon
+ * time) at the samples t_k + s*sample_time; filt = {b[4], a[4], lfilter_zi[3]} of
+ * butter(3, fc); mean, stdev [n_input].  Both halves integrate with classical RK4 on the
+ * linearly interpolated input (u_i; (u_i+u_i+1)/2 at both midpoints; u_i+1):
+ *   simulate: planned input + disturbance (white noise, Philox4x32-10 keyed by seed and
+ *             (step, instance, signal, sample), Box-Muller, filtfilt over n_traj samples)
+ *             -> first-order lag u' = (u_cmd - u)/time_constant from plant_u (lag != 0)
+ *             -> vehicle ODE from plant_x: plant_x_next, plant_u_next = last input sample
+ *   predict:  planned input -> vehicle ODE from plant_x: pred_x, pred_u = planned input at
+ *             sample n_samp.
+ * model: 0 integrator (Holonomic, Holonomic3D; input = ds/dt), 1 Quadrotor3D (thrust and
+ * angular rates from f~, q_phi, q_theta).  Rejected: other models, n_traj <= 12 with the
+ * disturbance (filtfilt's padding), time_constant <= 0 with the lag, null pointers. */
+int omg_closed_loop_step(int32_t model, int32_t B, int32_t n_state, int32_t n_input, int32_t n,
+                         const double* x, int32_t L, int32_t n_samp, const double* R0,
+                         const double* R1, double sample_time, int32_t lag, double time_constant,
+                         int32_t disturb, int32_t n_traj, const double* filt, const double* mean,
+                         const double* stdev, uint64_t seed, int32_t step, const double* plant_x,
+                         const double* plant_u, double* plant_x_next, double* plant_u_next,
+                         double* pred_x, double* pred_u, double* scratch, void* stream);
+
 /* ADMM consensus step for n_agents agents on the current device (DEVICE pointers):
  * closed-form z-update, lambda-update and squared residuals of the reference's
  * ADMM updater (omgtools/problems/admm.py:117-168 construct_upd_z/update_z,

@@ -1333,6 +1333,157 @@ __global__ void omg_rk4_kernel(int model, int B, int ns, int ni, const double* _
   for (int j = 0; j < ns; ++j) stateT[(size_t)b * ns + j] = x[j];
 }
 
+// ---- closed-loop plant step (reference Vehicle.simulate / predict without the ideal flags,
+// vehicle.py:302-337, 359-449) -----------------------------------------------------------------
+#define OMG_CL_MAX_INPUT 3
+#define OMG_CL_PAD 12          // filtfilt's odd padding: 3 * max(len(a), len(b)) for butter(3)
+
+// Philox4x32-10 (Salmon et al., "Parallel random numbers: as easy as 1, 2, 3", SC'11): counter
+// (sample pair, signal, instance, MPC step), key (seed).  A draw depends on its key and counter
+// only, so a realisation is the same at any batch size and under any launch schedule.
+__host__ __device__ __forceinline__ void omg_philox4x32_10(uint32_t c[4], uint32_t k0, uint32_t k1) {
+  for (int r = 0; r < 10; ++r) {
+    if (r) { k0 += 0x9E3779B9u; k1 += 0xBB67AE85u; }
+    const uint64_t p0 = (uint64_t)0xD2511F53u * c[0], p1 = (uint64_t)0xCD9E8D57u * c[2];
+    const uint32_t hi0 = (uint32_t)(p0 >> 32), lo0 = (uint32_t)p0, hi1 = (uint32_t)(p1 >> 32), lo1 = (uint32_t)p1;
+    c[0] = hi1 ^ c[1] ^ k0; c[1] = lo1; c[2] = hi0 ^ c[3] ^ k1; c[3] = lo0;
+  }
+}
+
+// two uniforms in (0, 1) from one Philox block (52 bits each, (m + 1/2) 2^-52, exact), then
+// Box-Muller: z0 = r cos(2 pi u2), z1 = r sin(2 pi u2), r = sqrt(-2 log u1)
+__device__ __forceinline__ void omg_normal_pair(uint64_t seed, int step, int inst, int sig, int pair,
+                                                double* z0, double* z1) {
+  uint32_t c[4] = {(uint32_t)pair, (uint32_t)sig, (uint32_t)inst, (uint32_t)step};
+  omg_philox4x32_10(c, (uint32_t)seed, (uint32_t)(seed >> 32));
+  const double u1 = ((double)(((((uint64_t)c[0] << 32) | c[1]) >> 12)) + 0.5) * 0x1p-52;
+  const double u2 = ((double)(((((uint64_t)c[2] << 32) | c[3]) >> 12)) + 0.5) * 0x1p-52;
+  const double r = sqrt(-2.0 * log(u1)), w = 6.283185307179586 * u2;
+  *z0 = r * cos(w);
+  *z1 = r * sin(w);
+}
+
+// One block per instance.  Both halves start from the plant state x_p(t_k) and the trajectory
+// just solved, sampled at t_k + s*dt, s = 0..n_samp:
+//   simulate: planned input + filtered noise -> first-order lag -> RK4 of the ODE -> x_p(t_k+1)
+//   predict:  planned input -> RK4 of the ODE from x_p(t_k) -> state0 of the next solve
+// RK4 takes the linearly interpolated input of the reference's interp1d: u_i, the mean of
+// u_i and u_i+1 at both midpoints, u_i+1 at the end.  The noise series of (instance, signal) is
+// filtered over the whole stored trajectory (n_traj samples) by the reference's
+// filtfilt(butter(3, fc)): odd extension by 12, forward and backward passes of the transposed
+// direct form from zi * (first value); only samples 0..n_samp are kept.
+// filt = {b0..b3, a0..a3 (a0 = 1), zi0..zi2}; scratch holds one forward pass per series.
+__global__ void omg_closed_loop_kernel(int model, int ns, int ni, int n, const double* __restrict__ x, int L,
+                                       int n_samp, const double* __restrict__ R0, const double* __restrict__ R1,
+                                       double dt, int lag, double tau, int disturb, int n_traj,
+                                       const double* __restrict__ filt, const double* __restrict__ mean,
+                                       const double* __restrict__ stdev, uint64_t seed, int step,
+                                       const double* plant_x, const double* plant_u,    // (may alias the next)
+                                       double* plant_x_next, double* plant_u_next,
+                                       double* __restrict__ pred_x, double* __restrict__ pred_u,
+                                       double* __restrict__ scratch) {
+  OMG_DYN_SHARED(sm);
+  const int b = blockIdx.x, ts = n_samp + 1;
+  double* U = sm;                // planned input [ts][ni]
+  double* D = sm + ts * ni;      // filtered disturbance [ts][ni]
+  double* A = sm + 2 * ts * ni;  // input reaching the ODE [ts][ni]
+  const double* xb = x + (size_t)b * n;
+  // planned inputs (holonomic*.py / quadrotor3d.py splines2signals); R1 rows carry the 1/T
+  for (int s = threadIdx.x; s < ts; s += blockDim.x) {
+    const double* r0 = R0 + (size_t)s * L;
+    const double* r1 = R1 + (size_t)s * L;
+    if (model == OMG_ODE_QUADROTOR3D) {
+      double f = 0.0, qp = 0.0, qt = 0.0, dqp = 0.0, dqt = 0.0;
+      for (int k = 0; k < L; ++k) {
+        f += r0[k] * xb[k]; qp += r0[k] * xb[L + k]; qt += r0[k] * xb[2 * L + k];
+        dqp += r1[k] * xb[L + k]; dqt += r1[k] * xb[2 * L + k];
+      }
+      const double ep = 1.0 + qp * qp, et = 1.0 + qt * qt;
+      U[s * 3] = f * (ep * et); U[s * 3 + 1] = 2.0 * dqp / ep; U[s * 3 + 2] = 2.0 * dqt / et;
+    } else {
+      for (int c = 0; c < ni; ++c) {
+        double acc = 0.0;
+        for (int k = 0; k < L; ++k) acc += r1[k] * xb[c * L + k];
+        U[s * ni + c] = acc;
+      }
+    }
+  }
+  if (disturb && (int)threadIdx.x < ni) {
+    const int j = threadIdx.x, N = n_traj + 2 * OMG_CL_PAD;
+    double* e = scratch + ((size_t)b * ni + j) * N;
+    double* w = e + OMG_CL_PAD;                     // white noise at 0..n_traj-1
+    for (int p = 0; 2 * p < n_traj; ++p) {
+      double z0, z1;
+      omg_normal_pair(seed, step, b, j, p, &z0, &z1);
+      w[2 * p] = mean[j] + stdev[j] * z0;
+      if (2 * p + 1 < n_traj) w[2 * p + 1] = mean[j] + stdev[j] * z1;
+    }
+    for (int i = 1; i <= OMG_CL_PAD; ++i) {         // odd extension (scipy odd_ext)
+      e[OMG_CL_PAD - i] = 2.0 * w[0] - w[i];
+      w[n_traj - 1 + i] = 2.0 * w[n_traj - 1] - w[n_traj - 1 - i];
+    }
+    const double b0 = filt[0], b1 = filt[1], b2 = filt[2], b3 = filt[3];
+    const double a1 = filt[5], a2 = filt[6], a3 = filt[7];
+    double z0 = filt[8] * e[0], z1 = filt[9] * e[0], z2 = filt[10] * e[0];
+    for (int i = 0; i < N; ++i) {                   // forward pass, in place
+      const double xi = e[i], yi = z0 + b0 * xi;
+      z0 = z1 + xi * b1 - yi * a1; z1 = z2 + xi * b2 - yi * a2; z2 = xi * b3 - yi * a3;
+      e[i] = yi;
+    }
+    const double y0 = e[N - 1];
+    z0 = filt[8] * y0; z1 = filt[9] * y0; z2 = filt[10] * y0;
+    for (int i = N - 1; i >= OMG_CL_PAD; --i) {     // backward pass down to sample 0
+      const double xi = e[i], yi = z0 + b0 * xi;
+      z0 = z1 + xi * b1 - yi * a1; z1 = z2 + xi * b2 - yi * a2; z2 = xi * b3 - yi * a3;
+      if (i - OMG_CL_PAD < ts) D[(i - OMG_CL_PAD) * ni + j] = yi;
+    }
+  }
+  double st[OMG_ODE_MAX_STATE], k1[OMG_ODE_MAX_STATE], k2[OMG_ODE_MAX_STATE], k3[OMG_ODE_MAX_STATE],
+         k4[OMG_ODE_MAX_STATE], y[OMG_ODE_MAX_STATE], um[OMG_CL_MAX_INPUT];
+  // read before the barrier: the outputs may overwrite the plant state in place
+  if (threadIdx.x <= 1)
+    for (int j = 0; j < ns; ++j) y[j] = plant_x[(size_t)b * ns + j];
+  __syncthreads();
+  if (threadIdx.x > 1) return;
+  const bool simulate = threadIdx.x == 0;
+  const double* Uin = U;
+  if (simulate) {
+    for (int i = 0; i < ts * ni; ++i) A[i] = disturb ? U[i] + D[i] : U[i];
+    if (lag) {                                      // u' = (u_cmd - u) / tau from the applied input
+      double ua[OMG_CL_MAX_INPUT];
+      for (int c = 0; c < ni; ++c) ua[c] = plant_u[(size_t)b * ni + c];
+      for (int i = 0; i < n_samp; ++i) {
+        for (int c = 0; c < ni; ++c) {
+          const double c0 = A[i * ni + c], c1 = A[(i + 1) * ni + c], cm = 0.5 * (c0 + c1), u = ua[c];
+          const double q1 = (c0 - u) / tau, q2 = (cm - (u + 0.5 * dt * q1)) / tau;
+          const double q3 = (cm - (u + 0.5 * dt * q2)) / tau, q4 = (c1 - (u + dt * q3)) / tau;
+          A[i * ni + c] = u;
+          ua[c] = u + (dt / 6.0) * (q1 + 2.0 * q2 + 2.0 * q3 + q4);
+        }
+      }
+      for (int c = 0; c < ni; ++c) A[n_samp * ni + c] = ua[c];
+    }
+    Uin = A;
+  }
+  for (int i = 0; i < n_samp; ++i) {
+    const double* u0 = Uin + i * ni;
+    const double* u1 = u0 + ni;
+    for (int c = 0; c < ni; ++c) um[c] = 0.5 * (u0[c] + u1[c]);
+    ode_rhs(model, ns, y, u0, k1);
+    for (int j = 0; j < ns; ++j) st[j] = y[j] + 0.5 * dt * k1[j];
+    ode_rhs(model, ns, st, um, k2);
+    for (int j = 0; j < ns; ++j) st[j] = y[j] + 0.5 * dt * k2[j];
+    ode_rhs(model, ns, st, um, k3);
+    for (int j = 0; j < ns; ++j) st[j] = y[j] + dt * k3[j];
+    ode_rhs(model, ns, st, u1, k4);
+    for (int j = 0; j < ns; ++j) y[j] += (dt / 6.0) * (k1[j] + 2.0 * k2[j] + 2.0 * k3[j] + k4[j]);
+  }
+  double* xo = simulate ? plant_x_next : pred_x;
+  double* uo = simulate ? plant_u_next : pred_u;
+  for (int j = 0; j < ns; ++j) xo[(size_t)b * ns + j] = y[j];
+  for (int c = 0; c < ni; ++c) uo[(size_t)b * ni + c] = Uin[n_samp * ni + c];
+}
+
 // trajectory sampling: out[b, blk, c, s] = sum_k S_blk[s,k] * x[b, off_blk + c*len_blk + k]
 // (batched Cox-de Boor evaluation with precomputed basis rows; reference
 //  Vehicle.store -> sample_splines, vehicle.py:250-300, spline_extra.py:406-410;
@@ -2437,6 +2588,53 @@ int omg_integrate_rk4(int32_t model, int32_t B, int32_t n_state, int32_t n_input
       n_state != want_s[model] || n_input != want_i[model]) { set_err("bad vehicle model / sizes"); return -1; }
   cudaStream_t stream = (cudaStream_t)stream_;
   OMG_LAUNCH(omg_rk4_kernel, (B + 127) / 128, 128, 0, stream, model, B, n_state, n_input, state0, inputs, sample_time, steps, stateT);
+  CK(cudaGetLastError());
+  return 0;
+}
+
+int omg_closed_loop_step(int32_t model, int32_t B, int32_t n_state, int32_t n_input, int32_t n, const double* x,
+                         int32_t L, int32_t n_samp, const double* R0, const double* R1, double sample_time,
+                         int32_t lag, double time_constant, int32_t disturb, int32_t n_traj, const double* filt,
+                         const double* mean, const double* stdev, uint64_t seed, int32_t step,
+                         const double* plant_x, const double* plant_u, double* plant_x_next, double* plant_u_next,
+                         double* pred_x, double* pred_u, double* scratch, void* stream_) {
+  if (model != OMG_ODE_INTEGRATOR && model != OMG_ODE_QUADROTOR3D) {
+    set_err("omg_closed_loop_step: unknown vehicle model " + std::to_string(model)); return -1; }
+  const bool sizes_ok = model == OMG_ODE_QUADROTOR3D ? (n_state == 8 && n_input == 3 && n >= 3 * L)
+                                                     : (n_state == n_input && n_input >= 1 &&
+                                                        n_input <= OMG_CL_MAX_INPUT && n >= n_input * L);
+  if (!sizes_ok || L < 1 || n_samp < 0) { set_err("omg_closed_loop_step: bad state / input / spline sizes"); return -1; }
+  // three [n_samp+1][n_input] arrays in the default 48 KB of dynamic shared memory
+  if ((int64_t)(n_samp + 1) * n_input > 2048) {
+    set_err("omg_closed_loop_step: (n_samp + 1) * n_input exceeds 2048 samples per update"); return -1; }
+  if (!(sample_time > 0.0)) { set_err("omg_closed_loop_step: sample_time must be > 0"); return -1; }
+  if (lag && !(time_constant > 0.0)) { set_err("omg_closed_loop_step: time_constant must be > 0 with the lag on"); return -1; }
+  if (disturb && n_traj <= OMG_CL_PAD) {
+    set_err("omg_closed_loop_step: n_traj must exceed the filter padding of 12 samples"); return -1; }
+  if (disturb && n_traj < n_samp + 1) { set_err("omg_closed_loop_step: n_traj < n_samp + 1"); return -1; }
+  if (!x || !R0 || !R1 || !plant_x || !plant_u || !plant_x_next || !plant_u_next || !pred_x || !pred_u ||
+      (disturb && (!filt || !mean || !stdev || !scratch))) { set_err("omg_closed_loop_step: null argument"); return -1; }
+  if (B <= 0) return 0;
+  cudaStream_t stream = (cudaStream_t)stream_;
+  // host descriptors -> device: R0 | R1 | filt (11) | mean | stdev
+  const size_t nr = (size_t)(n_samp + 1) * L;
+  std::vector<double> dv(2 * nr + 11 + 2 * (size_t)n_input, 0.0);
+  std::copy(R0, R0 + nr, dv.begin());
+  std::copy(R1, R1 + nr, dv.begin() + nr);
+  if (disturb) {
+    std::copy(filt, filt + 11, dv.begin() + 2 * nr);
+    std::copy(mean, mean + n_input, dv.begin() + 2 * nr + 11);
+    std::copy(stdev, stdev + n_input, dv.begin() + 2 * nr + 11 + n_input);
+  }
+  int device = 0;
+  CK(cudaGetDevice(&device));
+  static thread_local DescCache cache;
+  if (desc_upload(cache, device, std::vector<int>(1, 0), dv.data(), dv.size(), stream)) return -1;
+  const double* d = cache.d_d;
+  const size_t smem = sizeof(double) * 3 * (size_t)(n_samp + 1) * n_input;
+  OMG_LAUNCH(omg_closed_loop_kernel, B, 32, smem, stream, model, n_state, n_input, n, x, L, n_samp, d, d + nr,
+             sample_time, lag, time_constant, disturb, n_traj, d + 2 * nr, d + 2 * nr + 11, d + 2 * nr + 11 + n_input,
+             seed, step, plant_x, plant_u, plant_x_next, plant_u_next, pred_x, pred_u, scratch);
   CK(cudaGetLastError());
   return 0;
 }

@@ -4,8 +4,8 @@ every MPC step is ONE batched solve on the GPU.
 
 It is the batched counterpart of the reference's ``Simulator.run()`` /
 ``Deployer.update()`` loop (omgtools/execution/simulator.py:39-99,
-deployer.py:43-79) restricted to the ideal, noise-free case (the vehicle follows
-its spline; reference options ideal_prediction / ideal_update):
+deployer.py:43-79).  With the vehicle options ideal_prediction and ideal_update on
+(this repository's defaults) the vehicle follows its spline:
 
     per step:   predict  -> state0/input0 = spline and derivative at t + update_time
                 init_step-> knot-crossing shift T.dot(coeffs) of the seg0 variables
@@ -16,6 +16,17 @@ its spline; reference options ideal_prediction / ideal_update):
 
 The decision variables stay resident on the device between steps (warm start);
 only the parameter rows (n_par doubles per instance) travel each step.
+
+With either flag off (the reference's defaults) the loop is closed through the vehicle's
+own dynamics: after each solve ONE launch (omg_closed_loop_step) integrates the vehicle ODE
+from the plant state, once on the planned inputs plus the input disturbance and through the
+first-order actuator lag (simulate: the next plant state), once on the clean planned inputs
+(predict: state0 of the next solve).  Options read from the vehicle: ideal_update,
+ideal_prediction, 1storder_delay, time_constant, input_disturbance {fc, stdev, mean}; the noise
+is keyed by ``seed``, the MPC step and the instance, so a realisation does not depend on the
+batch size.  history['plant'] and history['plant_input'] hold the plant state and the last
+applied input at every update boundary.  ``sample_time`` is the simulation grid of the plant
+and of the obstacle motion (the reference simulator's sample_time, 0.01 s by default).
 """
 import numpy as np
 
@@ -150,6 +161,14 @@ class _Quadrotor3DAdapter(object):
         return self.state[:, :3]
 
 
+def plant_rows(basis, T, t_rel, sample_time, n_samp):
+    """Basis rows R0 and derivative rows R1 (divided by T) at t_rel + s * sample_time,
+    s = 0..n_samp: the samples of the stored trajectory that one update spans."""
+    tau = (t_rel + sample_time * np.arange(n_samp + 1)) / T
+    Bd, P1 = basis.derivative(1)
+    return basis.eval_basis(tau), Bd.eval_basis(tau).dot(P1) / T
+
+
 def _adapter_for(vehicle):
     name = type(vehicle).__name__
     if name in ('Holonomic', 'Holonomic3D'):
@@ -162,7 +181,7 @@ def _adapter_for(vehicle):
 class BatchMPC(object):
 
     def __init__(self, problem, batch, update_time=0.1, jitter=0.0, seed=0, device_predict=True,
-                 device=None):
+                 device=None, sample_time=0.01):
         import torch
         self.device_predict = device_predict
         self.torch = torch
@@ -212,6 +231,39 @@ class BatchMPC(object):
         self.time = 0.
         self.time_prev = 0.
         self.history = {'state': [self.state.copy()], 'iters': [], 'status': []}
+        self.sample_time = sample_time
+        opt = self.vehicle.options
+        self.ideal_update = opt.get('ideal_update', True)
+        self.ideal_prediction = opt.get('ideal_prediction', True)
+        self.closed_loop = not (self.ideal_update and self.ideal_prediction)
+        if self.closed_loop:
+            self._init_plant(opt, seed)
+
+    def _init_plant(self, opt, seed):
+        """Plant state and last applied input per instance (device tensors), the lag and the
+        disturbance of the vehicle's options, and the filter's scratch.  With ideal_update on the
+        plant follows the spline and the reference applies neither (vehicle.py:366-370)."""
+        from ..solver.b200 import ODE_MODELS, disturbance_filter
+        torch = self.torch
+        sample_time = self.sample_time
+        self.seed, self.k = seed, 0
+        self.model = ODE_MODELS[type(self.vehicle).__name__]
+        self.plant_x = torch.tensor(self.state, device=self.dev)
+        self.plant_u = torch.tensor(self.inp, device=self.dev)
+        self.pred_x, self.pred_u = torch.empty_like(self.plant_x), torch.empty_like(self.plant_u)
+        lag = opt.get('1storder_delay', False) and not self.ideal_update
+        self.time_constant = float(opt['time_constant']) if lag else None
+        self.disturbance = None
+        dist = opt.get('input_disturbance')
+        if dist and not self.ideal_update:
+            ni = self.plant_u.shape[1]
+            stdev = np.broadcast_to(np.asarray(dist['stdev'], dtype=float), (ni,))
+            mean = np.broadcast_to(np.asarray(dist.get('mean', np.zeros(ni)), dtype=float), (ni,))
+            n_traj = int(np.round(self.T / sample_time, 6)) + 1
+            scratch = torch.empty(self.B * ni * (n_traj + 24), dtype=torch.float64, device=self.dev)
+            self.disturbance = (disturbance_filter(dist['fc']), mean, stdev, scratch)
+        self.history['plant'] = [self.plant_x.cpu().numpy().copy()]
+        self.history['plant_input'] = [self.plant_u.cpu().numpy().copy()]
 
     # state / input / target of every instance (owned by the vehicle adapter)
     state = property(lambda self: self.veh.state)
@@ -231,7 +283,7 @@ class BatchMPC(object):
         P[:, off[(self.problem.label, 't')]] = np.round(t, 6) % self.knot_time
         P[:, off[(self.problem.label, 'T')]] = self.T
 
-    def _advance_obstacles(self, dt, sample_time=0.01):
+    def _advance_obstacles(self, dt, sample_time):
         """Obstacle motion over one update, sample by sample as the reference's
         simulator does it (obstacle.py:229-247): constant-acceleration steps plus the
         increments of the obstacle's 'trajectories' at their switching times."""
@@ -269,10 +321,42 @@ class BatchMPC(object):
         # ideal update: vehicle and obstacles move over update_time; the prediction at
         # t + update_time comes from spline values sampled on the device
         t_rel = np.round(t, 6) % self.knot_time
-        self.veh.predict(self.X, t_rel, self.update_time, self.T, device=self.device_predict)
-        self._advance_obstacles(self.update_time)
+        if self.closed_loop:
+            self._plant_step(t_rel)
+        else:
+            self.veh.predict(self.X, t_rel, self.update_time, self.T, device=self.device_predict)
+        self._advance_obstacles(self.update_time, self.sample_time)
         self.history['state'].append(self.state.copy())
         self.time = np.round(t + self.update_time, 6)
+
+    def _plant_step(self, t_rel):
+        """Reference Vehicle.simulate and predict (vehicle.py:302-337, 359-392) of every instance
+        in one launch; the ideal half of a mixed setting follows the spline as before."""
+        from ..solver.b200 import closed_loop_step
+        n_samp = int(np.round(self.update_time / self.sample_time, 6))
+        R0, R1 = plant_rows(self.vehicle.basis, self.T, t_rel, self.sample_time, n_samp)
+        dist = None
+        if self.disturbance is not None:
+            filt, mean, stdev, scratch = self.disturbance
+            n_traj = int(np.round((self.T - t_rel) / self.sample_time, 6)) + 1
+            dist = (filt, mean, stdev, n_traj, scratch)
+        closed_loop_step(self.model, self.X, len(self.vehicle.basis), R0, R1, self.sample_time,
+                         self.plant_x, self.plant_u,
+                         (self.plant_x, self.plant_u, self.pred_x, self.pred_u), self.k, seed=self.seed,
+                         time_constant=self.time_constant, disturbance=dist)
+        self.k += 1
+        if self.ideal_prediction or self.ideal_update:
+            self.veh.predict(self.X, t_rel, self.update_time, self.T, device=self.device_predict)
+        if self.ideal_update:
+            self.plant_x.copy_(self.torch.from_numpy(self.state))
+            self.plant_u.copy_(self.torch.from_numpy(self.inp))
+        if not self.ideal_prediction:
+            # (copies: the adapter updates its arrays in place, and on a CPU device .numpy()
+            # would share the kernel's output buffers)
+            self.veh.state = self.pred_x.cpu().numpy().copy()
+            self.veh.inp = self.pred_u.cpu().numpy().copy()
+        self.history['plant'].append(self.plant_x.cpu().numpy().copy())
+        self.history['plant_input'].append(self.plant_u.cpu().numpy().copy())
 
     def run(self, n_steps):
         for _ in range(n_steps):

@@ -267,6 +267,28 @@ def config_holonomic_orient(options=None, build_solver=True):
     return _p2p(vehicle, environment, options, build_solver)
 
 
+def config_disturbances(options=None, build_solver=True):
+    """examples/p2p_holonomic_disturbances.py: Holonomic with a first-order actuator lag
+    (time_constant 0.1) and a filtered input disturbance (fc 0.01, stdev 0.05), stop_tol 1e-2,
+    Square(5) room, two Rectangle(3, 0.2) walls and a Circle(0.4) that starts moving at t = 3 s.
+    The example keeps the reference's non-ideal vehicle defaults, so they are set here: the
+    closed loop runs in execution/batch_mpc.py (the host Vehicle.predict is ideal only)."""
+    vehicle = Holonomic()
+    vehicle.set_options({'safety_distance': 0.1, '1storder_delay': True, 'time_constant': 0.1,
+                         'input_disturbance': {'fc': 0.01, 'stdev': 0.05 * np.ones(2)},
+                         'stop_tol': 1.e-2, 'ideal_prediction': False, 'ideal_update': False})
+    vehicle.set_initial_conditions([-1.5, -1.5])
+    vehicle.set_terminal_conditions([2., 2.])
+    environment = Environment(room={'shape': Square(5.)})
+    rectangle = Rectangle(width=3., height=0.2)
+    environment.add_obstacle(Obstacle({'position': [-2.1, -0.5]}, shape=rectangle))
+    environment.add_obstacle(Obstacle({'position': [1.7, -0.5]}, shape=rectangle))
+    trajectories = {'velocity': {'time': [3., 4.], 'values': [[-0.15, 0.0], [0., 0.15]]}}
+    environment.add_obstacle(Obstacle({'position': [1.5, 0.5]}, shape=Circle(0.4),
+                                      simulation={'trajectories': trajectories}))
+    return _p2p(vehicle, environment, options, build_solver)
+
+
 def config_freeT(options=None, build_solver=True, moving=False):
     """Minimum-time variant of examples/p2p_holonomic.py (freeT=True, the
     example's commented alternative): two rectangular walls and a circle

@@ -86,7 +86,7 @@ EXPORTS = ['omg_abi_version', 'omg_last_error', 'omg_default_options',
            'omg_admm_zl_update', 'omg_sample_batch', 'omg_tables_read',
            'omg_tables_free', 'omg_integrate_rk4', 'omg_feas_batch', 'omg_feas_batch_host',
            'omg_comm_unique_id', 'omg_comm_create', 'omg_comm_destroy', 'omg_admm_exchange_x',
-           'omg_admm_zl_update_dist']
+           'omg_admm_zl_update_dist', 'omg_closed_loop_step']
 
 _lib = None
 
@@ -140,6 +140,9 @@ def bind(lib):
     lib.omg_admm_zl_update.argtypes = [C.c_int32] * 4 + [vp] * 4 + [C.c_double] + [vp] * 8
     lib.omg_sample_batch.argtypes = [C.c_int32, C.c_int32, vp, C.c_int32] + [vp] * 7
     lib.omg_integrate_rk4.argtypes = [C.c_int32] * 4 + [vp, vp, C.c_double, C.c_int32, vp, vp]
+    lib.omg_closed_loop_step.argtypes = ([C.c_int32] * 5 + [vp, C.c_int32, C.c_int32, vp, vp, C.c_double,
+                                         C.c_int32, C.c_double, C.c_int32, C.c_int32, vp, vp, vp,
+                                         C.c_uint64, C.c_int32] + [vp] * 8)
     lib.omg_tables_read.argtypes = [C.c_char_p]
     lib.omg_tables_read.restype = C.POINTER(_Tables)
     lib.omg_tables_free.argtypes = [C.POINTER(_Tables)]
@@ -675,3 +678,55 @@ def integrate_rk4(model, state0, inputs, sample_time, stream=None):
     if rc != 0:
         raise RuntimeError('libomgb200: %s' % lib.omg_last_error().decode())
     return out
+
+
+def disturbance_filter(fc):
+    """{b, a, lfilter_zi} of the reference's input-disturbance filter butter(3, fc, 'low')
+    (vehicle.py:444), flattened as omg_closed_loop_step takes it."""
+    from scipy.signal import butter, lfilter_zi
+    b, a = butter(3, fc, 'low')
+    return np.ascontiguousarray(np.r_[b, a, lfilter_zi(b, a)], dtype=np.float64)
+
+
+def closed_loop_step(model, X, L, R0, R1, sample_time, plant_x, plant_u, out, step, seed=0,
+                     time_constant=None, disturbance=None, stream=None):
+    """Plant step of MPC step ``step`` for a batch (omg_closed_loop_step): the non-ideal
+    simulate and predict of the reference's Vehicle from the plant state / last applied input
+    (plant_x [B, n_state], plant_u [B, n_input]) along the trajectories of the spline
+    coefficients X [B, n], sampled by the host rows R0, R1 [n_samp+1, L].
+    out = (plant_x_next, plant_u_next, pred_x, pred_u), written in place (the plant outputs may
+    be plant_x / plant_u themselves).  time_constant: first-order actuator lag (None = off).
+    disturbance: (filt, mean, stdev, n_traj, scratch) with filt from disturbance_filter(fc) and
+    scratch a float64 tensor of at least B * n_input * (n_traj + 24) elements (None = off)."""
+    lib = load_library()
+    mid = ODE_MODELS[model] if isinstance(model, str) else int(model)
+    tensors = (X, plant_x, plant_u) + tuple(out)
+    if disturbance is not None:
+        filt, mean, stdev, n_traj, scratch = disturbance
+        tensors += (scratch,)
+        if scratch.numel() < X.shape[0] * plant_u.shape[1] * (n_traj + 24):
+            raise ValueError('disturbance scratch too small')
+        filt, mean, stdev = (np.ascontiguousarray(a, dtype=np.float64) for a in (filt, mean, stdev))
+        if filt.size != 11 or mean.size != plant_u.shape[1] or stdev.size != plant_u.shape[1]:
+            raise ValueError('disturbance filter / mean / stdev sizes')
+    on_gpu = _check_device_tensors(tensors, lib)
+    B, ns = plant_x.shape
+    ni = plant_u.shape[1]
+    R0 = np.ascontiguousarray(R0, dtype=np.float64)
+    R1 = np.ascontiguousarray(R1, dtype=np.float64)
+    if R0.shape != R1.shape or R0.ndim != 2 or R0.shape[1] != L:
+        raise ValueError('R0 / R1 must both be [n_samp + 1, L]')
+    for t, shape in zip(out, ((B, ns), (B, ni), (B, ns), (B, ni))):
+        if tuple(t.shape) != shape:
+            raise ValueError('output tensor shapes do not match the plant state / input')
+    d = disturbance is not None
+    rc = lib.omg_closed_loop_step(
+        mid, B, ns, ni, X.shape[1], X.data_ptr(), L, R0.shape[0] - 1, R0.ctypes.data, R1.ctypes.data,
+        float(sample_time), int(time_constant is not None),
+        float(time_constant) if time_constant is not None else 0., int(d), int(n_traj) if d else 0,
+        filt.ctypes.data if d else None, mean.ctypes.data if d else None,
+        stdev.ctypes.data if d else None, int(seed) & 0xFFFFFFFFFFFFFFFF, int(step),
+        plant_x.data_ptr(), plant_u.data_ptr(), *[t.data_ptr() for t in out],
+        scratch.data_ptr() if d else None, _stream_handle(on_gpu, X.device, stream))
+    if rc != 0:
+        raise RuntimeError('libomgb200: %s' % lib.omg_last_error().decode())
