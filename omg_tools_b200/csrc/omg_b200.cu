@@ -89,11 +89,6 @@ struct DevTab {
   const int2* midg; const int* jtptr; const int* jrow;
   const int *jp_ptr, *jp_a, *jp_c, *mu_ptr, *mu_row, *mu_slot;
   const int* jxvar; int n_jxvar;       // extra J slots with an x factor (the others are constant in a solve)
-  // J^T Sigma J gather by row chunks staged in shared memory (XL kernel, Jacobian values in scratch):
-  // chunk c = the slots [hc_slot[c], hc_slot[c+1]) of whole rows; virtual thread vt owns H positions;
-  // its k-th record of chunk c sits at hc_rec[hc_base[c] + k * hc_vt + vt] = {dst, s1 | s2<<16} (chunk-relative)
-  int hc_nchunk, hc_vt;
-  const int *hc_slot, *hc_base, *hc_cnt; const uint2* hc_rec;
   // extra Hessian slots (mid coefficient depends on x or on another mid): wrec[nnz_w ..
   // nnz_w+nnz_wx) hold the term ranges, xq the H positions that gather
   // sum Wx[e.x] * Jx[e.y] * (e.z >= 0 ? Jx[e.z] : 1)
@@ -106,7 +101,6 @@ struct Smem {                      // offsets in doubles
   int sgn, eptr, efirst, pptr, prow, pcmin;
   int arr[N_ARR];                  // >= 0: shared offset; < 0: -(scratch offset + 1)
   int LDP, total;
-  int hst, hch;                    // staging buffer of the chunked H gather: 2 x hch doubles at hst
   int Kg, Vg, jxg, mug, Kcg, wxg;  // XL kernel: scratch offsets (K only if S.K < 0)
 };
 
@@ -830,38 +824,6 @@ __device__ __forceinline__ void ipm_body(const DevTab& T, const omg_options& O, 
         }
         __syncthreads();
         // H positions: gather J^T Sigma J (+ delta_w on the diagonal)
-        if (XL && T.hc_nchunk > 0) {
-          // the Jacobian values live in the L2-resident scratch: a pair would cost two scattered
-          // 8-byte loads (32-byte sectors).  Instead the rows are staged chunk by chunk into the
-          // panel buffers (free until the factorisation) with coalesced loads, and every thread
-          // adds the pairs of ITS H positions that fall into the chunk, from a coalesced record
-          // stream (positions are owned by one virtual thread, so no atomics).
-          double* Ach = sm + S.hst; double* Bch = Ach + S.hch;
-          for (int c = 0; c < T.hc_nchunk; ++c) {
-            const int s0 = T.hc_slot[c], nsl = T.hc_slot[c + 1] - s0;
-            for (int k = tid; k < nsl; k += NT) { Ach[k] = jval[s0 + k]; Bch[k] = jsv[s0 + k]; }
-            __syncthreads();
-            const uint2* rp = T.hc_rec + (size_t)T.hc_base[c];
-            for (int vt = tid; vt < T.hc_vt; vt += NT) {
-              const int cnt = T.hc_cnt[c * T.hc_vt + vt];
-              unsigned cur = 0xffffffffu;
-              double acc = 0.0;
-              for (int k0 = 0; k0 < cnt; k0 += 8) {        // eight record loads in flight
-                uint2 r[8];
-#pragma unroll
-                for (int u = 0; u < 8; ++u) if (k0 + u < cnt) r[u] = __ldg(rp + (size_t)(k0 + u) * T.hc_vt + vt);
-#pragma unroll
-                for (int u = 0; u < 8; ++u) if (k0 + u < cnt) {
-                  if (r[u].x != cur) { if (cur != 0xffffffffu) K[cur] += acc; cur = r[u].x; acc = 0.0; }
-                  acc += Bch[r[u].y & 0xffffu] * Ach[r[u].y >> 16];
-                }
-              }
-              if (cur != 0xffffffffu) K[cur] += acc;
-            }
-            __syncthreads();
-          }
-          for (int j = tid; j < n; j += NT) K[T.kdiag[T.pos_var[j]]] += ctl.delta_w;
-        } else
         for (int q = tid; q < T.nnz_h; q += NT) {
           const HqRec h = T.hq[q];
           double acc = 0.0;
@@ -911,8 +873,7 @@ __device__ __forceinline__ void ipm_body(const DevTab& T, const omg_options& O, 
           for (int t = w.t0; t < w.t1; ++t) {
             int lr;
             double v = term_value(T.Wt + t, V, xe, &lr);
-            if (XL) v *= (lr < m) ? (y[lr] * dsc[lr]) : (lr == m ? ctl.fsc : mu_mid[lr - m - 1]);
-            else v *= (lr < m) ? (y[lr] * dsc[lr]) : ctl.fsc;
+            v *= (lr < m) ? (y[lr] * dsc[lr]) : ctl.fsc;
             acc += v;
           }
           K[w.dst] += acc;
@@ -2155,13 +2116,11 @@ omg_problem* omg_problem_create(const omg_tables* tb, const omg_options* opt, in
     if (cudaFuncGetAttributes(&fx, (const void*)omg_ipm_kernel_xl) == cudaSuccess)
       bx = (size_t)prop.sharedMemPerBlockOptin - fx.sharedSizeBytes;
     h->xl = (n_mid > 0) || layout(true, true) > b0;
-    const char* kg = getenv("OMG_B200_XL_KGLOBAL");   // tuning knob: 1 = K in scratch even if it fits
-    const bool kglob = kg && atoi(kg) == 1;
     if (h->xl) {
       // what is read at random stays on the SM in this order: K, then the parameter tape V (one
       // load per TERM of every stream); the m-vectors are streamed one thread per row and go last
-      if (!kglob && layout(true, true) <= bx) { }
-      else if (!kglob && layout(true, false) <= bx) { }
+      if (layout(true, true) <= bx) { }
+      else if (layout(true, false) <= bx) { }
       else { k_in_smem = false; if (layout(false, true) > bx) layout(false, false); }
     } else layout(true, true);
   }
@@ -2198,16 +2157,6 @@ omg_problem* omg_problem_create(const omg_tables* tb, const omg_options* opt, in
   }
   S.Kcg = goff; goff += (T.env_size + 2 + 1) & ~1;
   const int sizes[N_ARR] = {tb->nnz_j, m, tb->nnz_j, m, m, m, m, m, m, m, m, m, m, m, m, m, m, m, m};
-  // staging buffer of the chunked J^T Sigma J gather (XL kernel with the Jacobian values in
-  // scratch): the panel buffers by default; three quarters of the free shared memory (up to
-  // 2 x 4096 doubles) when that is more -- fewer, longer chunks; the streamed m-vectors take the rest
-  S.hst = S.Pt; S.hch = NB * S.LDP;
-  if (h->xl && getenv("OMG_B200_HCHUNK") && atoi(getenv("OMG_B200_HCHUNK")) == 1 &&
-      (size_t)(off + 2 * ((tb->nnz_j + 1) & ~1)) * 8 > budget) {
-    const long long free_d = ((long long)budget - (long long)off * 8) / 8;
-    int ch = (int)std::min<long long>(4096, (free_d * 3 / 4) / 2) & ~1;
-    if (ch > S.hch) { S.hst = off; S.hch = ch; off += 2 * ch; }
-  }
   for (int k = 0; k < N_ARR; ++k) {
     const int cnt = (sizes[k] + 1) & ~1;
     const bool optional_low = (k >= A_ZL);     // lower-bound / equality-only arrays: rarely touched
@@ -2215,80 +2164,6 @@ omg_problem* omg_problem_create(const omg_tables* tb, const omg_options* opt, in
     else { S.arr[k] = -(goff + 1); goff += cnt; }
   }
   S.total = off;
-  T.hc_nchunk = 0; T.hc_vt = 0;
-  // (experimental, off by default: OMG_B200_HCHUNK=1.  It changes the summation order, which the
-  //  300-600-iteration cold starts of HolonomicOrient amplify to 3e-4)
-  const char* hce = getenv("OMG_B200_HCHUNK");
-  if (ok && hce && atoi(hce) == 1 && h->xl && S.arr[A_JVAL] < 0 && S.arr[A_JSV] < 0 && tb->nnz_h > 0) {
-    // chunked J^T Sigma J gather (see the kernel): chunks of whole rows that fit one panel buffer
-    const int CH = std::min(S.hch, 65535), VT = 512;
-    std::vector<int> cslot(1, 0), chunk_of_row(m, 0);
-    bool fits = true;
-    int cur0 = 0;
-    for (int i = 0; i < m && fits; ++i) {
-      const int a = tb->jrow_ptr[i], b = tb->jrow_ptr[i + 1];
-      if (b - a > CH) fits = false;
-      if (b - cur0 > CH) { cslot.push_back(a); cur0 = a; }
-      chunk_of_row[i] = (int)cslot.size() - 1;
-    }
-    cslot.push_back(tb->nnz_j);
-    if (fits) {
-      const int nc = (int)cslot.size() - 1;
-      // per chunk: the pairs of every H position that fall into it, positions dealt to the
-      // virtual threads by pair count (LPT).  A position may change hands between chunks: the
-      // chunks are separated by barriers.
-      std::vector<std::vector<std::vector<uint2>>> per(nc);     // [chunk][position in chunk] -> records
-      {
-        std::vector<int> slot_in_chunk(tb->nnz_h, -1);
-        for (int c = 0; c < nc; ++c) per[c].clear();
-        std::vector<int> last_chunk(tb->nnz_h, -1);
-        for (int q = 0; q < tb->nnz_h; ++q)
-          for (int e = tb->hp_ptr[q]; e < tb->hp_ptr[q + 1]; ++e) {
-            const int c = chunk_of_row[tb->hp_row[e]];
-            if (last_chunk[q] != c) { last_chunk[q] = c; slot_in_chunk[q] = (int)per[c].size(); per[c].push_back({}); }
-            per[c][slot_in_chunk[q]].push_back(make_uint2((unsigned)tb->kkt_hdst[q],
-                (unsigned)(tb->hp_s1[e] - cslot[c]) | ((unsigned)(tb->hp_s2[e] - cslot[c]) << 16)));
-          }
-      }
-      std::vector<std::vector<uint2>> lists((size_t)nc * VT);
-      typedef std::pair<long long, int> LT;
-      for (int c = 0; c < nc; ++c) {
-        std::vector<int> ord(per[c].size());
-        for (size_t k = 0; k < ord.size(); ++k) ord[k] = (int)k;
-        std::stable_sort(ord.begin(), ord.end(), [&](int a, int b) { return per[c][a].size() > per[c][b].size(); });
-        std::priority_queue<LT, std::vector<LT>, std::greater<LT>> heap;
-        for (int t = 0; t < VT; ++t) heap.push(LT(0, t));
-        for (int k : ord) {
-          LT top = heap.top(); heap.pop();
-          std::vector<uint2>& dst = lists[(size_t)c * VT + top.second];
-          dst.insert(dst.end(), per[c][k].begin(), per[c][k].end());
-          heap.push(LT(top.first + (long long)per[c][k].size(), top.second));
-        }
-      }
-      std::vector<int> base(nc), cnt((size_t)nc * VT);
-      size_t total = 0;
-      for (int c = 0; c < nc; ++c) {
-        size_t mx = 0;
-        for (int t = 0; t < VT; ++t) { cnt[(size_t)c * VT + t] = (int)lists[(size_t)c * VT + t].size(); mx = std::max(mx, lists[(size_t)c * VT + t].size()); }
-        base[c] = (int)total; total += mx * VT;
-      }
-      std::vector<uint2> rec(std::max<size_t>(total, 1), make_uint2(0u, 0u));
-      for (int c = 0; c < nc; ++c)
-        for (int t = 0; t < VT; ++t) {
-          const std::vector<uint2>& l = lists[(size_t)c * VT + t];
-          for (size_t k = 0; k < l.size(); ++k) rec[(size_t)base[c] + k * VT + t] = l[k];
-        }
-      if (total < (size_t)1 << 31) {
-        T.hc_slot = upload(h, cslot.data(), cslot.size(), &ok);
-        T.hc_base = upload(h, base.data(), base.size(), &ok);
-        T.hc_cnt = upload(h, cnt.data(), cnt.size(), &ok);
-        T.hc_rec = upload(h, rec.data(), rec.size(), &ok);
-        T.hc_nchunk = nc; T.hc_vt = VT;
-        if (getenv("OMG_B200_VERBOSE"))
-          fprintf(stderr, "[omg_b200] chunked H gather: %d chunks of <= %d slots, %d pairs, %zu record slots\n", nc, CH, tb->n_hp, total);
-      }
-    }
-  }
   h->smem_bytes = (size_t)off * sizeof(double);
   if (ok && cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                  (int)((size_t)prop.sharedMemPerBlockOptin - fa.sharedSizeBytes)) != cudaSuccess) {

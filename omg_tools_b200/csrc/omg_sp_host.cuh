@@ -100,10 +100,8 @@ static bool sp_symbolic(const omg_tables* tb, SpSym& Y, std::string* why) {
   // symbolic structure stays closed and the padded entries stay exactly zero), are numbered
   // consecutively and are scheduled as ONE level step: gather from outside, then a dense
   // (w + rows) x w panel finished without block-wide barriers (omg_sp.cuh, sp_factor).
-  int snw_max = SP_SNW;
-  int snz_max = SP_SNZ;                       // (both: tuning knobs for experiments)
+  int snw_max = SP_SNW;                       // (tuning knob for experiments)
   { const char* e = getenv("OMG_B200_SNW"); if (e && atoi(e) >= 1 && atoi(e) <= SP_SNW) snw_max = atoi(e); }
-  { const char* e = getenv("OMG_B200_SNZ"); if (e && atoi(e) >= 0) snz_max = atoi(e); }
   std::vector<int> sn_id(R0, -1);
   std::vector<std::vector<int>> paths;
   int total_z = 0;
@@ -119,7 +117,7 @@ static bool sp_symbolic(const omg_tables* tb, SpSym& Y, std::string* why) {
       const int L = (int)path.size() + 1;
       int newz = 0;
       for (int q = 0; q < L - 1; ++q) newz += (L - 1 - q) + (int)Y.st[p].size() - (int)Y.st[path[q]].size();
-      if (newz > snz_max || total_z + newz - zcur > SP_SNZ_TOTAL) break;
+      if (newz > SP_SNZ || total_z + newz - zcur > SP_SNZ_TOTAL) break;
       path.push_back(p); sn_id[p] = id;
       total_z += newz - zcur; zcur = newz;
     }

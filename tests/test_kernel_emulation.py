@@ -149,28 +149,6 @@ def test_xl_kernel_config4(emu):
     assert abs(res['f'][0] - ref['f'][0]) < 1e-7
 
 
-def test_xl_chunked_gather_option_agrees_with_the_default(emu, monkeypatch):
-    """OMG_B200_HCHUNK=1: the J^T Sigma J gather of the XL kernel by row chunks staged in shared
-    memory (off by default, DESIGN.md section 3b) -- another summation order of the same assembly:
-    the nominal instance step for step (59 iterations, 7e-7), a jittered one within an iteration
-    and tol-size (1.4e-3: this NLP amplifies rounding, tests/test_gpu_parity.py -- the reason the
-    option is off by default)."""
-    X0, P = None, None
-    out = []
-    for flag in (None, '1'):
-        if flag:
-            monkeypatch.setenv('OMG_B200_HCHUNK', flag)
-        pr = sc.config4()
-        if X0 is None:
-            X0, P = sc.instance_data(pr, 2, jitter=0.05, seed=3)
-            X0[0], P[0] = sc.instance_data(pr, 1)[0][0], sc.instance_data(pr, 1)[1][0]
-        out.append(pr.problem.solve_batch(X0, P))
-    a, b = out
-    assert np.array_equal(a['status'], b['status']) and (a['status'] == 0).all()
-    assert a['iters'][0] == b['iters'][0] and abs(int(a['iters'][1]) - int(b['iters'][1])) <= 2
-    assert np.abs(a['x'] - b['x'])[0].max() < 1e-6 and np.abs(a['x'] - b['x'])[:, :36].max() < 5e-3
-
-
 def test_xl_kernel_cross_hessian_dubins_default(emu):
     """The cross-Hessian slots of the XL kernel (Dubins without substitution: hyperplane
     normal times integrated position; include/omg_b200.h xq_*): identical path on the
