@@ -255,7 +255,9 @@ int omg_sample_batch(int32_t B, int32_t n, const double* x, int32_t n_blocks,
  * stages at the initial state, the running state is used (identical for the holonomic
  * integrator model).  model: 0 integrator (state' = input: Holonomic, Holonomic1D/3D),
  * 1 Quadrotor3D (8 states, 3 inputs; quadrotor3d.py:308-312), 2 planar Quadrotor
- * (5 states, 2 inputs; quadrotor.py:154-157). */
+ * (5 states, 2 inputs; quadrotor.py:154-157), 3 Dubins (3 states, 2 inputs: x' = v cos theta,
+ * y' = v sin theta, theta' = omega), 4 HolonomicOrient (integrator, 3 states and inputs),
+ * 5 SimpleQuadrotor3D (Quadrotor3D's 8 states, 3 inputs and ODE). */
 int omg_integrate_rk4(int32_t model, int32_t B, int32_t n_state, int32_t n_input,
                       const double* state0, const double* inputs, double sample_time,
                       int32_t steps, double* stateT, void* stream);
@@ -286,6 +288,34 @@ int omg_closed_loop_step(int32_t model, int32_t B, int32_t n_state, int32_t n_in
                          const double* stdev, uint64_t seed, int32_t step, const double* plant_x,
                          const double* plant_u, double* plant_x_next, double* plant_u_next,
                          double* pred_x, double* pred_u, double* scratch, void* stream);
+
+/* omg_closed_loop_step for every vehicle model with a planned-input map, the ones that need
+ * higher derivatives of the flat outputs included.  The derivative rows come as ONE host array
+ * R [n_der x (n_samp+1) x L]: row d is the d-th derivative of the basis divided by T^d at the
+ * samples t_k + s*sample_time (n_der from 2 to 4: value, first, second, third derivative).
+ * Every other argument, the outputs and the integration are omg_closed_loop_step's, which
+ * forwards here with n_der = 2 (results bit-identical).  Models and the planned input they
+ * take from the spline columns (the vehicle's splines2signals; g = 9.81), n_state / n_input,
+ * the n_der they need, and the ODE:
+ *   0 integrator  (Holonomic, Holonomic3D)  n / n  2  input = ds/dt; s' = input
+ *   1 Quadrotor3D  8 / 3  2  thrust and angular rates from f~, q_phi, q_theta
+ *   2 Quadrotor    5 / 2  4  u1 = sqrt(x''^2 + (y''+g)^2),
+ *                            u2 = (x'''(y''+g) - x'' y''') / ((y''+g)^2 + x''^2); quadrotor.py ode
+ *   3 Dubins       3 / 2  2  v = v~ (1 + tg^2), omega = 2 tg' / (1 + tg^2);
+ *                            (v cos theta, v sin theta, omega)
+ *   4 HolonomicOrient 3 / 3  2  (x', y', 2 tg' / (1 + tg^2)); integrator
+ *   5 SimpleQuadrotor3D 8 / 3  4  u1, u2, u3 of quadrotor3d_simple.py (az = z'' + g);
+ *                            Quadrotor3D's ODE
+ * Rejected with a message: unknown models, sizes that do not match the model, n_der below the
+ * model's or above 4, and everything omg_closed_loop_step rejects. */
+int omg_closed_loop_step_der(int32_t model, int32_t B, int32_t n_state, int32_t n_input, int32_t n,
+                             const double* x, int32_t L, int32_t n_samp, int32_t n_der,
+                             const double* R, double sample_time, int32_t lag,
+                             double time_constant, int32_t disturb, int32_t n_traj,
+                             const double* filt, const double* mean, const double* stdev,
+                             uint64_t seed, int32_t step, const double* plant_x,
+                             const double* plant_u, double* plant_x_next, double* plant_u_next,
+                             double* pred_x, double* pred_u, double* scratch, void* stream);
 
 /* ADMM consensus step for n_agents agents on the current device (DEVICE pointers):
  * closed-form z-update, lambda-update and squared residuals of the reference's

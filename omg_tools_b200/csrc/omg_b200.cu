@@ -1248,19 +1248,41 @@ __global__ void omg_shift_kernel(double* x, int B, int n, int n_blocks, const in
   }
 }
 
-// vehicle models for the batched state prediction (reference Vehicle.ode of each class)
-enum { OMG_ODE_INTEGRATOR = 0, OMG_ODE_QUADROTOR3D = 1, OMG_ODE_QUADROTOR2D = 2 };
+// vehicle models for the batched state prediction and the closed-loop plant step (reference
+// Vehicle.ode and splines2signals of each class)
+enum { OMG_ODE_INTEGRATOR = 0, OMG_ODE_QUADROTOR3D = 1, OMG_ODE_QUADROTOR2D = 2, OMG_ODE_DUBINS = 3,
+       OMG_ODE_HOLONOMIC_ORIENT = 4, OMG_ODE_SIMPLE_QUADROTOR3D = 5, OMG_ODE_N_MODELS = 6 };
 #define OMG_ODE_MAX_STATE 8
 
-__device__ __forceinline__ void ode_rhs(int model, int ns, const double* st, const double* u, double* d) {
-  if (model == OMG_ODE_QUADROTOR3D) {          // quadrotor3d.py:308-312
+// Per model: state and input sizes (0: any, with n_state = n_input), the rows of spline
+// derivatives its planned input reads (value and first derivative = 2; the input splines are
+// its first n_input spline columns), and the right-hand side it integrates.
+struct OmgOdeModel { int n_state, n_input, n_der, ode; };
+static const OmgOdeModel omg_ode_models[OMG_ODE_N_MODELS] = {
+  {0, 0, 2, OMG_ODE_INTEGRATOR},      // Holonomic, Holonomic1D, Holonomic3D
+  {8, 3, 2, OMG_ODE_QUADROTOR3D},     // Quadrotor3D
+  {5, 2, 4, OMG_ODE_QUADROTOR2D},     // Quadrotor
+  {3, 2, 2, OMG_ODE_DUBINS},          // Dubins
+  {3, 3, 2, OMG_ODE_INTEGRATOR},      // HolonomicOrient: (x, y, theta)' = input
+  {8, 3, 4, OMG_ODE_QUADROTOR3D},     // SimpleQuadrotor3D: Quadrotor3D's state and ODE
+};
+
+static bool omg_ode_sizes_ok(int model, int n_state, int n_input) {
+  const OmgOdeModel& m = omg_ode_models[model];
+  return m.n_state ? (n_state == m.n_state && n_input == m.n_input) : (n_state == n_input && n_input >= 1);
+}
+
+__device__ __forceinline__ void ode_rhs(int ode, int ns, const double* st, const double* u, double* d) {
+  if (ode == OMG_ODE_QUADROTOR3D) {            // quadrotor3d.py:308-312, quadrotor3d_simple.py:186-190
     const double phi = st[6], theta = st[7], g = 9.81;
     d[0] = st[3]; d[1] = st[4]; d[2] = st[5];
     d[3] = u[0] * sin(theta) * cos(phi); d[4] = -u[0] * sin(phi);
     d[5] = -g + u[0] * cos(phi) * cos(theta); d[6] = u[1]; d[7] = u[2];
-  } else if (model == OMG_ODE_QUADROTOR2D) {   // quadrotor.py:154-157
+  } else if (ode == OMG_ODE_QUADROTOR2D) {     // quadrotor.py:154-157
     const double theta = st[4], g = 9.81;
     d[0] = st[2]; d[1] = st[3]; d[2] = u[0] * sin(theta); d[3] = u[0] * cos(theta) - g; d[4] = u[1];
+  } else if (ode == OMG_ODE_DUBINS) {          // dubins.py: (v cos theta, v sin theta, omega)
+    d[0] = u[0] * cos(st[2]); d[1] = u[0] * sin(st[2]); d[2] = u[1];
   } else {                                     // holonomic*.py: state' = input
     for (int j = 0; j < ns; ++j) d[j] = u[j];
   }
@@ -1324,6 +1346,12 @@ __device__ __forceinline__ void omg_normal_pair(uint64_t seed, int step, int ins
   *z1 = r * sin(w);
 }
 
+__device__ __forceinline__ double omg_row_dot(const double* r, const double* c, int L) {
+  double acc = 0.0;
+  for (int k = 0; k < L; ++k) acc += r[k] * c[k];
+  return acc;
+}
+
 // One block per instance.  Both halves start from the plant state x_p(t_k) and the trajectory
 // just solved, sampled at t_k + s*dt, s = 0..n_samp:
 //   simulate: planned input + filtered noise -> first-order lag -> RK4 of the ODE -> x_p(t_k+1)
@@ -1334,8 +1362,10 @@ __device__ __forceinline__ void omg_normal_pair(uint64_t seed, int step, int ins
 // filtfilt(butter(3, fc)): odd extension by 12, forward and backward passes of the transposed
 // direct form from zi * (first value); only samples 0..n_samp are kept.
 // filt = {b0..b3, a0..a3 (a0 = 1), zi0..zi2}; scratch holds one forward pass per series.
-__global__ void omg_closed_loop_kernel(int model, int ns, int ni, int n, const double* __restrict__ x, int L,
-                                       int n_samp, const double* __restrict__ R0, const double* __restrict__ R1,
+// R = [n_der][n_samp+1][L]: row d is the d-th derivative of the basis divided by T^d.  `model`
+// selects the planned-input map, `ode` the right-hand side (omg_ode_models).
+__global__ void omg_closed_loop_kernel(int model, int ode, int ns, int ni, int n, const double* __restrict__ x,
+                                       int L, int n_samp, const double* __restrict__ R,
                                        double dt, int lag, double tau, int disturb, int n_traj,
                                        const double* __restrict__ filt, const double* __restrict__ mean,
                                        const double* __restrict__ stdev, uint64_t seed, int step,
@@ -1349,11 +1379,36 @@ __global__ void omg_closed_loop_kernel(int model, int ns, int ni, int n, const d
   double* D = sm + ts * ni;      // filtered disturbance [ts][ni]
   double* A = sm + 2 * ts * ni;  // input reaching the ODE [ts][ni]
   const double* xb = x + (size_t)b * n;
-  // planned inputs (holonomic*.py / quadrotor3d.py splines2signals); R1 rows carry the 1/T
+  // planned inputs (splines2signals of each vehicle); row d carries the 1/T^d
+  const size_t nr = (size_t)ts * L;
   for (int s = threadIdx.x; s < ts; s += blockDim.x) {
-    const double* r0 = R0 + (size_t)s * L;
-    const double* r1 = R1 + (size_t)s * L;
-    if (model == OMG_ODE_QUADROTOR3D) {
+    const double* r0 = R + (size_t)s * L;
+    const double* r1 = r0 + nr;
+    if (model == OMG_ODE_QUADROTOR2D) {             // quadrotor.py splines2signals
+      const double *r2 = r0 + 2 * nr, *r3 = r0 + 3 * nr;
+      const double ddx = omg_row_dot(r2, xb, L), ddy = omg_row_dot(r2, xb + L, L);
+      const double dddx = omg_row_dot(r3, xb, L), dddy = omg_row_dot(r3, xb + L, L);
+      const double ay = ddy + 9.81;
+      U[s * 2] = sqrt(ddx * ddx + ay * ay);
+      U[s * 2 + 1] = (dddx * ay - ddx * dddy) / (ay * ay + ddx * ddx);
+    } else if (model == OMG_ODE_DUBINS) {           // dubins.py: v = v~ (1 + tg^2), w = 2 tg' / (1 + tg^2)
+      const double vt = omg_row_dot(r0, xb, L), tg = omg_row_dot(r0, xb + L, L);
+      const double dtg = omg_row_dot(r1, xb + L, L), q = 1.0 + tg * tg;
+      U[s * 2] = vt * q; U[s * 2 + 1] = 2.0 * dtg / q;
+    } else if (model == OMG_ODE_HOLONOMIC_ORIENT) { // holonomicorient.py: (x', y', 2 tg' / (1 + tg^2))
+      const double tg = omg_row_dot(r0, xb + 2 * L, L);
+      U[s * 3] = omg_row_dot(r1, xb, L); U[s * 3 + 1] = omg_row_dot(r1, xb + L, L);
+      U[s * 3 + 2] = 2.0 * omg_row_dot(r1, xb + 2 * L, L) / (1.0 + tg * tg);
+    } else if (model == OMG_ODE_SIMPLE_QUADROTOR3D) {   // quadrotor3d_simple.py splines2signals
+      const double *r2 = r0 + 2 * nr, *r3 = r0 + 3 * nr;
+      const double ddx = omg_row_dot(r2, xb, L), ddy = omg_row_dot(r2, xb + L, L);
+      const double dddx = omg_row_dot(r3, xb, L), dddy = omg_row_dot(r3, xb + L, L);
+      const double az = omg_row_dot(r2, xb + 2 * L, L) + 9.81, dddz = omg_row_dot(r3, xb + 2 * L, L);
+      const double h2 = ddx * ddx + az * az, f2 = ddx * ddx + ddy * ddy + az * az;
+      U[s * 3] = sqrt(f2);
+      U[s * 3 + 1] = (-dddy * h2 + ddy * (ddx * dddx + dddz * az)) / (f2 * sqrt(h2));
+      U[s * 3 + 2] = (az * dddx - ddx * dddz) / (az * az + ddx * ddx);
+    } else if (model == OMG_ODE_QUADROTOR3D) {
       double f = 0.0, qp = 0.0, qt = 0.0, dqp = 0.0, dqt = 0.0;
       for (int k = 0; k < L; ++k) {
         f += r0[k] * xb[k]; qp += r0[k] * xb[L + k]; qt += r0[k] * xb[2 * L + k];
@@ -1430,13 +1485,13 @@ __global__ void omg_closed_loop_kernel(int model, int ns, int ni, int n, const d
     const double* u0 = Uin + i * ni;
     const double* u1 = u0 + ni;
     for (int c = 0; c < ni; ++c) um[c] = 0.5 * (u0[c] + u1[c]);
-    ode_rhs(model, ns, y, u0, k1);
+    ode_rhs(ode, ns, y, u0, k1);
     for (int j = 0; j < ns; ++j) st[j] = y[j] + 0.5 * dt * k1[j];
-    ode_rhs(model, ns, st, um, k2);
+    ode_rhs(ode, ns, st, um, k2);
     for (int j = 0; j < ns; ++j) st[j] = y[j] + 0.5 * dt * k2[j];
-    ode_rhs(model, ns, st, um, k3);
+    ode_rhs(ode, ns, st, um, k3);
     for (int j = 0; j < ns; ++j) st[j] = y[j] + dt * k3[j];
-    ode_rhs(model, ns, st, u1, k4);
+    ode_rhs(ode, ns, st, u1, k4);
     for (int j = 0; j < ns; ++j) y[j] += (dt / 6.0) * (k1[j] + 2.0 * k2[j] + 2.0 * k3[j] + k4[j]);
   }
   double* xo = simulate ? plant_x_next : pred_x;
@@ -2458,48 +2513,54 @@ int omg_integrate_rk4(int32_t model, int32_t B, int32_t n_state, int32_t n_input
                       const double* inputs, double sample_time, int32_t steps, double* stateT, void* stream_) {
   if (B <= 0) return 0;
   if (!state0 || !inputs || !stateT) { set_err("null buffer"); return -1; }
-  const int want_s[3] = {n_input, 8, 5}, want_i[3] = {n_input, 3, 2};
-  if (model < 0 || model > 2 || n_state < 1 || n_state > OMG_ODE_MAX_STATE || steps < 0 ||
-      n_state != want_s[model] || n_input != want_i[model]) { set_err("bad vehicle model / sizes"); return -1; }
+  if (model < 0 || model >= OMG_ODE_N_MODELS || n_state < 1 || n_state > OMG_ODE_MAX_STATE || steps < 0 ||
+      !omg_ode_sizes_ok(model, n_state, n_input)) { set_err("bad vehicle model / sizes"); return -1; }
   cudaStream_t stream = (cudaStream_t)stream_;
-  OMG_LAUNCH(omg_rk4_kernel, (B + 127) / 128, 128, 0, stream, model, B, n_state, n_input, state0, inputs, sample_time, steps, stateT);
+  OMG_LAUNCH(omg_rk4_kernel, (B + 127) / 128, 128, 0, stream, omg_ode_models[model].ode, B, n_state, n_input,
+             state0, inputs, sample_time, steps, stateT);
   CK(cudaGetLastError());
   return 0;
 }
 
-int omg_closed_loop_step(int32_t model, int32_t B, int32_t n_state, int32_t n_input, int32_t n, const double* x,
-                         int32_t L, int32_t n_samp, const double* R0, const double* R1, double sample_time,
-                         int32_t lag, double time_constant, int32_t disturb, int32_t n_traj, const double* filt,
-                         const double* mean, const double* stdev, uint64_t seed, int32_t step,
-                         const double* plant_x, const double* plant_u, double* plant_x_next, double* plant_u_next,
-                         double* pred_x, double* pred_u, double* scratch, void* stream_) {
-  if (model != OMG_ODE_INTEGRATOR && model != OMG_ODE_QUADROTOR3D) {
-    set_err("omg_closed_loop_step: unknown vehicle model " + std::to_string(model)); return -1; }
-  const bool sizes_ok = model == OMG_ODE_QUADROTOR3D ? (n_state == 8 && n_input == 3 && n >= 3 * L)
-                                                     : (n_state == n_input && n_input >= 1 &&
-                                                        n_input <= OMG_CL_MAX_INPUT && n >= n_input * L);
-  if (!sizes_ok || L < 1 || n_samp < 0) { set_err("omg_closed_loop_step: bad state / input / spline sizes"); return -1; }
+// omg_closed_loop_step and omg_closed_loop_step_der; `fn` names the caller in the messages.  R
+// holds the rows [n_der][n_samp+1][L], except row 1 when R1 is given (omg_closed_loop_step's
+// separate R0 and R1).
+static int closed_loop_launch(const char* fn, int32_t model, int32_t B, int32_t n_state, int32_t n_input, int32_t n,
+                              const double* x, int32_t L, int32_t n_samp, int32_t n_der, const double* R,
+                              const double* R1, double sample_time, int32_t lag, double time_constant, int32_t disturb, int32_t n_traj,
+                              const double* filt, const double* mean, const double* stdev, uint64_t seed,
+                              int32_t step, const double* plant_x, const double* plant_u, double* plant_x_next,
+                              double* plant_u_next, double* pred_x, double* pred_u, double* scratch, void* stream_) {
+  const std::string f(fn);
+  if (model < 0 || model >= OMG_ODE_N_MODELS) { set_err(f + ": unknown vehicle model " + std::to_string(model)); return -1; }
+  const bool sizes_ok = omg_ode_sizes_ok(model, n_state, n_input) && n_input <= OMG_CL_MAX_INPUT && n >= n_input * L;
+  if (!sizes_ok || L < 1 || n_samp < 0) { set_err(f + ": bad state / input / spline sizes"); return -1; }
+  if (n_der < omg_ode_models[model].n_der || n_der > 4) {
+    set_err(f + ": vehicle model " + std::to_string(model) + " needs " + std::to_string(omg_ode_models[model].n_der) +
+            " to 4 derivative rows, got " + std::to_string(n_der)); return -1; }
   // three [n_samp+1][n_input] arrays in the default 48 KB of dynamic shared memory
   if ((int64_t)(n_samp + 1) * n_input > 2048) {
-    set_err("omg_closed_loop_step: (n_samp + 1) * n_input exceeds 2048 samples per update"); return -1; }
-  if (!(sample_time > 0.0)) { set_err("omg_closed_loop_step: sample_time must be > 0"); return -1; }
-  if (lag && !(time_constant > 0.0)) { set_err("omg_closed_loop_step: time_constant must be > 0 with the lag on"); return -1; }
+    set_err(f + ": (n_samp + 1) * n_input exceeds 2048 samples per update"); return -1; }
+  if (!(sample_time > 0.0)) { set_err(f + ": sample_time must be > 0"); return -1; }
+  if (lag && !(time_constant > 0.0)) { set_err(f + ": time_constant must be > 0 with the lag on"); return -1; }
   if (disturb && n_traj <= OMG_CL_PAD) {
-    set_err("omg_closed_loop_step: n_traj must exceed the filter padding of 12 samples"); return -1; }
-  if (disturb && n_traj < n_samp + 1) { set_err("omg_closed_loop_step: n_traj < n_samp + 1"); return -1; }
-  if (!x || !R0 || !R1 || !plant_x || !plant_u || !plant_x_next || !plant_u_next || !pred_x || !pred_u ||
-      (disturb && (!filt || !mean || !stdev || !scratch))) { set_err("omg_closed_loop_step: null argument"); return -1; }
+    set_err(f + ": n_traj must exceed the filter padding of 12 samples"); return -1; }
+  if (disturb && n_traj < n_samp + 1) { set_err(f + ": n_traj < n_samp + 1"); return -1; }
+  if (!x || !R || !plant_x || !plant_u || !plant_x_next || !plant_u_next || !pred_x || !pred_u ||
+      (disturb && (!filt || !mean || !stdev || !scratch))) { set_err(f + ": null argument"); return -1; }
   if (B <= 0) return 0;
   cudaStream_t stream = (cudaStream_t)stream_;
-  // host descriptors -> device: R0 | R1 | filt (11) | mean | stdev
-  const size_t nr = (size_t)(n_samp + 1) * L;
-  std::vector<double> dv(2 * nr + 11 + 2 * (size_t)n_input, 0.0);
-  std::copy(R0, R0 + nr, dv.begin());
-  std::copy(R1, R1 + nr, dv.begin() + nr);
+  // host descriptors -> device: R (the rows the model reads) | filt (11) | mean | stdev
+  const size_t nr = (size_t)(n_samp + 1) * L, nR = (size_t)omg_ode_models[model].n_der * nr;
+  std::vector<double> dv(nR + 11 + 2 * (size_t)n_input, 0.0);
+  for (int r = 0; r < omg_ode_models[model].n_der; ++r) {
+    const double* src = r == 1 && R1 ? R1 : R + r * nr;
+    std::copy(src, src + nr, dv.begin() + r * nr);
+  }
   if (disturb) {
-    std::copy(filt, filt + 11, dv.begin() + 2 * nr);
-    std::copy(mean, mean + n_input, dv.begin() + 2 * nr + 11);
-    std::copy(stdev, stdev + n_input, dv.begin() + 2 * nr + 11 + n_input);
+    std::copy(filt, filt + 11, dv.begin() + nR);
+    std::copy(mean, mean + n_input, dv.begin() + nR + 11);
+    std::copy(stdev, stdev + n_input, dv.begin() + nR + 11 + n_input);
   }
   int device = 0;
   CK(cudaGetDevice(&device));
@@ -2507,11 +2568,36 @@ int omg_closed_loop_step(int32_t model, int32_t B, int32_t n_state, int32_t n_in
   if (desc_upload(cache, device, std::vector<int>(1, 0), dv.data(), dv.size(), stream)) return -1;
   const double* d = cache.d_d;
   const size_t smem = sizeof(double) * 3 * (size_t)(n_samp + 1) * n_input;
-  OMG_LAUNCH(omg_closed_loop_kernel, B, 32, smem, stream, model, n_state, n_input, n, x, L, n_samp, d, d + nr,
-             sample_time, lag, time_constant, disturb, n_traj, d + 2 * nr, d + 2 * nr + 11, d + 2 * nr + 11 + n_input,
-             seed, step, plant_x, plant_u, plant_x_next, plant_u_next, pred_x, pred_u, scratch);
+  OMG_LAUNCH(omg_closed_loop_kernel, B, 32, smem, stream, model, omg_ode_models[model].ode, n_state, n_input, n, x,
+             L, n_samp, d, sample_time, lag, time_constant, disturb, n_traj, d + nR, d + nR + 11,
+             d + nR + 11 + n_input, seed, step, plant_x, plant_u, plant_x_next, plant_u_next, pred_x, pred_u, scratch);
   CK(cudaGetLastError());
   return 0;
+}
+
+int omg_closed_loop_step_der(int32_t model, int32_t B, int32_t n_state, int32_t n_input, int32_t n, const double* x,
+                             int32_t L, int32_t n_samp, int32_t n_der, const double* R, double sample_time,
+                             int32_t lag, double time_constant, int32_t disturb, int32_t n_traj, const double* filt,
+                             const double* mean, const double* stdev, uint64_t seed, int32_t step,
+                             const double* plant_x, const double* plant_u, double* plant_x_next,
+                             double* plant_u_next, double* pred_x, double* pred_u, double* scratch, void* stream) {
+  return closed_loop_launch("omg_closed_loop_step_der", model, B, n_state, n_input, n, x, L, n_samp, n_der, R,
+                            nullptr, sample_time, lag, time_constant, disturb, n_traj, filt, mean, stdev, seed, step, plant_x,
+                            plant_u, plant_x_next, plant_u_next, pred_x, pred_u, scratch, stream);
+}
+
+int omg_closed_loop_step(int32_t model, int32_t B, int32_t n_state, int32_t n_input, int32_t n, const double* x,
+                         int32_t L, int32_t n_samp, const double* R0, const double* R1, double sample_time,
+                         int32_t lag, double time_constant, int32_t disturb, int32_t n_traj, const double* filt,
+                         const double* mean, const double* stdev, uint64_t seed, int32_t step,
+                         const double* plant_x, const double* plant_u, double* plant_x_next, double* plant_u_next,
+                         double* pred_x, double* pred_u, double* scratch, void* stream) {
+  if (model != OMG_ODE_INTEGRATOR && model != OMG_ODE_QUADROTOR3D) {
+    set_err("omg_closed_loop_step: unknown vehicle model " + std::to_string(model)); return -1; }
+  if (!R1) R0 = nullptr;                            // (reported as a null argument)
+  return closed_loop_launch("omg_closed_loop_step", model, B, n_state, n_input, n, x, L, n_samp, 2, R0, R1,
+                            sample_time, lag, time_constant, disturb, n_traj, filt, mean, stdev, seed, step, plant_x,
+                            plant_u, plant_x_next, plant_u_next, pred_x, pred_u, scratch, stream);
 }
 
 int omg_admm_zl_update(int32_t n_agents, int32_t nsh, int32_t n_nghb, int32_t L,

@@ -1,5 +1,6 @@
 """Batched receding-horizon driver: B independent copies of one Point2point
-scenario (Holonomic, Holonomic3D or Quadrotor3D vehicle) advance in lock step,
+scenario (Holonomic, Holonomic3D, Quadrotor3D, Dubins, HolonomicOrient, planar Quadrotor or
+SimpleQuadrotor3D vehicle) advance in lock step,
 every MPC step is ONE batched solve on the GPU.
 
 It is the batched counterpart of the reference's ``Simulator.run()`` /
@@ -34,6 +35,8 @@ import numpy as np
 class _HolonomicAdapter(object):
     """Holonomic / Holonomic3D: state = position spline value, input = its
     derivative / T (holonomic.py:87-105, 153-159)."""
+
+    N_DER = 2       # rows of spline derivatives the plant step reads (value, first derivative)
 
     def __init__(self, mpc, vehicle, batch, jitter, rng):
         self.mpc, self.v = mpc, vehicle
@@ -88,6 +91,7 @@ class _Quadrotor3DAdapter(object):
     Gauss-Legendre quadrature per knot piece on device-sampled spline values."""
 
     NQ = 6      # exact for the degree-9 integrand (tau1 - s) * ddx(s)
+    N_DER = 2
 
     def __init__(self, mpc, vehicle, batch, jitter, rng):
         self.mpc, self.v = mpc, vehicle
@@ -161,6 +165,234 @@ class _Quadrotor3DAdapter(object):
         return self.state[:, :3]
 
 
+def _rows(basis, tau, T, n_der):
+    """Rows of the basis and of its derivatives 1..n_der-1 at tau, derivative d divided by
+    T^d: [n_der, len(tau), L]."""
+    rows = [basis.eval_basis(tau)]
+    for d in range(1, n_der):
+        Bd, Pd = basis.derivative(d)
+        rows.append(Bd.eval_basis(tau).dot(Pd) / T**d)
+    return np.array(rows)
+
+
+def _sample(X, L, n_col, S, device):
+    """Spline columns 0..n_col-1 of every instance at the rows S [n_rows, L]: [B, n_col * n_rows]
+    laid out column / row (on the device by omg_sample_batch, or on the host)."""
+    from ..solver.b200 import sample_batch
+    if device:
+        return sample_batch(X, [(0, L, n_col, S)]).cpu().numpy()
+    Xh = X.cpu().numpy()
+    return np.concatenate([Xh[:, k * L:(k + 1) * L].dot(S.T) for k in range(n_col)], axis=1)
+
+
+def _put(P, off, label, name, val):
+    val = np.asarray(val, dtype=float)
+    val = val[:, None] if val.ndim == 1 else val
+    P[:, off[(label, name)]:off[(label, name)] + val.shape[1]] = val
+
+
+class _DubinsAdapter(object):
+    """Dubins (dubins.py, every formulation): the decision splines are v~ and tg = tan(theta/2);
+    the position is the running integral of v~ (1 - tg^2), 2 v~ tg re-anchored at the previous
+    prediction (splines2signals, integrate_once).  The integral over one update is taken exactly
+    by Gauss-Legendre quadrature per knot piece on device-sampled spline values."""
+
+    N_DER = 2
+
+    def __init__(self, mpc, vehicle, batch, jitter, rng):
+        self.mpc, self.v = mpc, vehicle
+        rep = lambda a: np.repeat(np.asarray(a, float)[None], batch, 0)
+        self.state, self.inp = rep(vehicle.prediction['state']), rep(vehicle.prediction['input'])
+        self.poseT = rep(vehicle.poseT)
+        if jitter > 0:
+            self.state[1:, :2] += rng.uniform(-jitter, jitter, (batch - 1, 2))
+            self.poseT[1:, :2] += rng.uniform(-jitter, jitter, (batch - 1, 2))
+        self.nq = (3 * vehicle.degree + 2) // 2     # exact for the degree-3d integrand
+
+    def cold_start(self, X0):
+        L = len(self.v.basis)
+        X0[:, :L] = self.v.options.get('init_v_til', 0.)
+        X0[:, L:2 * L] = np.linspace(np.tan(self.state[:, 2] / 2.), np.tan(self.poseT[:, 2] / 2.), L).T
+
+    def pack(self, P, off):
+        v, st, inp = self.v.label, self.state, self.inp
+        tg = np.tan(st[:, 2] / 2.)
+        _put(P, off, v, 'tg_ha0', tg)
+        _put(P, off, v, 'v_til0', inp[:, 0] / (1 + tg**2))
+        _put(P, off, v, 'dtg_ha0', 0.5 * inp[:, 1] * (1 + tg**2))
+        _put(P, off, v, 'pos0', st[:, :2])
+        _put(P, off, v, 'posT', self.poseT[:, :2])
+        _put(P, off, v, 'tg_haT', np.tan(self.poseT[:, 2] / 2.))
+
+    def predict(self, X, t_rel, dt, T, device=True):
+        basis = self.v.basis
+        L = len(basis)
+        tau0, tau1 = t_rel / T, (t_rel + dt) / T
+        brk = [tau0] + [k for k in np.unique(basis.knots) if tau0 + 1e-12 < k < tau1 - 1e-12] + [tau1]
+        xg, wg = np.polynomial.legendre.leggauss(self.nq)
+        nodes = np.concatenate([0.5 * (b - a) * xg + 0.5 * (a + b) for a, b in zip(brk[:-1], brk[1:])])
+        wts = np.concatenate([0.5 * (b - a) * wg for a, b in zip(brk[:-1], brk[1:])])
+        R = _rows(basis, [tau1], T, 2)
+        nn = len(nodes)
+        out = _sample(X, L, 2, np.vstack([basis.eval_basis(nodes), R[0], R[1]]), device)
+        vt, tg = out[:, :nn], out[:, nn + 2:2 * nn + 2]
+        vt1, tg1, dtg1 = out[:, nn], out[:, 2 * nn + 2], out[:, 2 * nn + 3]
+        q1 = 1 + tg1**2
+        self.state = np.c_[self.state[:, 0] + T * (vt * (1 - tg**2)).dot(wts),
+                           self.state[:, 1] + T * (vt * (2 * tg)).dot(wts), 2 * np.arctan2(tg1, 1)]
+        self.inp = np.c_[vt1 * q1, 2 * dtg1 / q1]
+
+    def position(self):
+        return self.state[:, :2]
+
+
+class _HolonomicOrientAdapter(object):
+    """HolonomicOrient (holonomicorient.py): x, y and tg = tan(theta/2) are the decision splines;
+    state (x, y, theta), input (x', y', theta')."""
+
+    N_DER = 2
+
+    def __init__(self, mpc, vehicle, batch, jitter, rng):
+        self.mpc, self.v = mpc, vehicle
+        rep = lambda a: np.repeat(np.asarray(a, float)[None], batch, 0)
+        self.state, self.inp = rep(vehicle.prediction['state']), rep(vehicle.prediction['input'])
+        self.poseT = rep(vehicle.poseT)
+        if jitter > 0:
+            self.state[1:, :2] += rng.uniform(-jitter, jitter, (batch - 1, 2))
+            self.poseT[1:, :2] += rng.uniform(-jitter, jitter, (batch - 1, 2))
+
+    def cold_start(self, X0):
+        L = len(self.v.basis)
+        for k in range(2):
+            X0[:, k * L:(k + 1) * L] = np.linspace(self.state[:, k], self.poseT[:, k], L).T
+        X0[:, 2 * L:3 * L] = 0.
+
+    def pack(self, P, off):
+        v, st, inp = self.v.label, self.state, self.inp
+        tg = np.tan(st[:, 2] / 2)
+        _put(P, off, v, 'pos0', st[:, :2])
+        _put(P, off, v, 'tg_ha0', tg)
+        _put(P, off, v, 'vel0', inp[:, :2])
+        _put(P, off, v, 'dtg_ha0', 0.5 * inp[:, 2] * (1 + tg**2))
+        _put(P, off, v, 'posT', self.poseT[:, :2])
+        _put(P, off, v, 'tg_haT', np.tan(self.poseT[:, 2] / 2))
+
+    def predict(self, X, t_rel, dt, T, device=True):
+        basis = self.v.basis
+        R = _rows(basis, [(t_rel + dt) / T], T, 2)
+        out = _sample(X, len(basis), 3, np.vstack([R[0], R[1]]), device)   # column: value, derivative
+        tg, dtg = out[:, 4], out[:, 5]
+        self.state = np.c_[out[:, 0], out[:, 2], 2 * np.arctan2(tg, 1)]
+        self.inp = np.c_[out[:, 1], out[:, 3], 2 * dtg / (1 + tg**2)]
+
+    def position(self):
+        return self.state[:, :2]
+
+
+class _QuadrotorAdapter(object):
+    """Planar Quadrotor (quadrotor.py): the position splines x, y are the flat outputs; state
+    (x, y, x', y', theta), input (thrust, pitch rate) and the spline derivatives dspl, ddspl of
+    set_parameters follow from the derivatives up to the third (splines2signals)."""
+
+    N_DER = 4
+
+    def __init__(self, mpc, vehicle, batch, jitter, rng):
+        self.mpc, self.v = mpc, vehicle
+        rep = lambda a: np.repeat(np.asarray(a, float)[None], batch, 0)
+        self.state, self.inp = rep(vehicle.prediction['state']), rep(vehicle.prediction['input'])
+        self.dspl, self.ddspl = rep(vehicle.prediction['dspl']), rep(vehicle.prediction['ddspl'])
+        self.poseT = rep(vehicle.poseT)
+        if jitter > 0:
+            self.state[1:, :2] += rng.uniform(-jitter, jitter, (batch - 1, 2))
+            self.poseT[1:, :2] += rng.uniform(-jitter, jitter, (batch - 1, 2))
+
+    def cold_start(self, X0):
+        L, d = len(self.v.basis), self.v.degree
+        for k in range(2):
+            p0, pT = self.state[:, k:k + 1], self.poseT[:, k:k + 1]
+            X0[:, k * L:(k + 1) * L] = np.c_[np.repeat(p0, d, 1), np.linspace(p0[:, 0], pT[:, 0], L - 2 * d).T,
+                                             np.repeat(pT, d, 1)]
+
+    def pack(self, P, off):
+        v = self.v.label
+        _put(P, off, v, 'spl0', self.state[:, :2])
+        _put(P, off, v, 'dspl0', self.dspl)
+        _put(P, off, v, 'ddspl0', self.ddspl)
+        _put(P, off, v, 'poseT', self.poseT)
+
+    def _signals(self, X, tau1, T, device):
+        """x, y and their derivatives 1..3 at tau1: [B, 2 (column), 4 (derivative)]."""
+        basis = self.v.basis
+        out = _sample(X, len(basis), 2, _rows(basis, [tau1], T, 4)[:, 0], device)
+        return out.reshape(-1, 2, 4)
+
+    def predict(self, X, t_rel, dt, T, device=True):
+        s, g = self._signals(X, (t_rel + dt) / T, T, device), self.v.g
+        (x, dx, ddx, dddx), (y, dy, ddy, dddy) = s[:, 0].T, s[:, 1].T
+        self.state = np.c_[x, y, dx, dy, np.arctan2(ddx, ddy + g)]
+        self.inp = np.c_[np.sqrt(ddx**2 + (ddy + g)**2),
+                         (dddx * (ddy + g) - ddx * dddy) / ((ddy + g)**2 + ddx**2)]
+        self.dspl, self.ddspl = s[:, :, 1].copy(), s[:, :, 2].copy()
+
+    def predict_planned(self, X, t_rel, dt, T, device=True):
+        """The signals that the non-ideal prediction still takes from the planned trajectory
+        (reference vehicle.py:326-328): dspl and ddspl at t + dt."""
+        s = self._signals(X, (t_rel + dt) / T, T, device)
+        self.dspl, self.ddspl = s[:, :, 1].copy(), s[:, :, 2].copy()
+
+    def position(self):
+        return self.state[:, :2]
+
+
+class _SimpleQuadrotor3DAdapter(object):
+    """SimpleQuadrotor3D (quadrotor3d_simple.py): the position splines x, y, z are the flat
+    outputs; state (position, velocity, roll, pitch) and input (thrust, roll and pitch rates)
+    follow from the derivatives up to the third (splines2signals)."""
+
+    N_DER = 4
+
+    def __init__(self, mpc, vehicle, batch, jitter, rng):
+        self.mpc, self.v = mpc, vehicle
+        rep = lambda a: np.repeat(np.asarray(a, float)[None], batch, 0)
+        self.state, self.inp = rep(vehicle.prediction['state']), rep(vehicle.prediction['input'])
+        self.poseT = rep(vehicle.positionT)
+        if jitter > 0:
+            self.state[1:, :3] += rng.uniform(-jitter, jitter, (batch - 1, 3))
+            self.poseT[1:, :3] += rng.uniform(-jitter, jitter, (batch - 1, 3))
+
+    def cold_start(self, X0):
+        L = len(self.v.basis)
+        for k in range(3):
+            X0[:, k * L:(k + 1) * L] = np.linspace(self.state[:, k], self.poseT[:, k], L).T
+
+    def pack(self, P, off):
+        v, st, g = self.v.label, self.state, self.v.g
+        f0, phi0, theta0 = self.inp[:, 0], st[:, 6], st[:, 7]
+        _put(P, off, v, 'spl0', st[:, :3])
+        _put(P, off, v, 'ddspl0', np.c_[f0 * np.cos(phi0) * np.sin(theta0), -f0 * np.sin(phi0),
+                                        f0 * np.cos(phi0) * np.cos(theta0) - g])
+        _put(P, off, v, 'dspl0', st[:, 3:6])
+        _put(P, off, v, 'positionT', self.poseT)
+
+    def predict(self, X, t_rel, dt, T, device=True):
+        basis, g = self.v.basis, self.v.g
+        s = _sample(X, len(basis), 3, _rows(basis, [(t_rel + dt) / T], T, 4)[:, 0], device).reshape(-1, 3, 4)
+        pos, vel = s[:, :, 0], s[:, :, 1]
+        (ddx, ddy, ddz), (dddx, dddy, dddz) = s[:, :, 2].T, s[:, :, 3].T
+        az = ddz + g
+        phi = np.arctan2(-ddy, np.sqrt(ddx**2 + az**2))
+        theta = np.arctan2(ddx, az)
+        u1 = np.sqrt(ddx**2 + ddy**2 + az**2)
+        u2 = (-dddy * (ddx**2 + az**2) + ddy * (ddx * dddx + dddz * az)) / \
+            ((ddx**2 + ddy**2 + az**2) * np.sqrt(ddx**2 + az**2))
+        u3 = (az * dddx - ddx * dddz) / (az**2 + ddx**2)
+        self.state = np.c_[pos, vel, phi, theta]
+        self.inp = np.c_[u1, u2, u3]
+
+    def position(self):
+        return self.state[:, :3]
+
+
 def plant_rows(basis, T, t_rel, sample_time, n_samp):
     """Basis rows R0 and derivative rows R1 (divided by T) at t_rel + s * sample_time,
     s = 0..n_samp: the samples of the stored trajectory that one update spans."""
@@ -169,13 +401,25 @@ def plant_rows(basis, T, t_rel, sample_time, n_samp):
     return basis.eval_basis(tau), Bd.eval_basis(tau).dot(P1) / T
 
 
+def plant_rows_der(basis, T, t_rel, sample_time, n_samp):
+    """plant_rows and the rows of the second and third derivative (divided by T^2, T^3) at the
+    same samples: [4, n_samp + 1, L], the layout of omg_closed_loop_step_der."""
+    tau = (t_rel + sample_time * np.arange(n_samp + 1)) / T
+    return np.concatenate([np.array(plant_rows(basis, T, t_rel, sample_time, n_samp)),
+                           _rows(basis, tau, T, 4)[2:]])
+
+
+_ADAPTERS = {'Holonomic': _HolonomicAdapter, 'Holonomic3D': _HolonomicAdapter,
+             'Quadrotor3D': _Quadrotor3DAdapter, 'Dubins': _DubinsAdapter,
+             'HolonomicOrient': _HolonomicOrientAdapter, 'Quadrotor': _QuadrotorAdapter,
+             'SimpleQuadrotor3D': _SimpleQuadrotor3DAdapter}
+
+
 def _adapter_for(vehicle):
     name = type(vehicle).__name__
-    if name in ('Holonomic', 'Holonomic3D'):
-        return _HolonomicAdapter
-    if name == 'Quadrotor3D':
-        return _Quadrotor3DAdapter
-    raise NotImplementedError('BatchMPC has no batched prediction for %s' % name)
+    if name not in _ADAPTERS:
+        raise NotImplementedError('BatchMPC has no batched prediction for %s' % name)
+    return _ADAPTERS[name]
 
 
 class BatchMPC(object):
@@ -334,7 +578,12 @@ class BatchMPC(object):
         in one launch; the ideal half of a mixed setting follows the spline as before."""
         from ..solver.b200 import closed_loop_step
         n_samp = int(np.round(self.update_time / self.sample_time, 6))
-        R0, R1 = plant_rows(self.vehicle.basis, self.T, t_rel, self.sample_time, n_samp)
+        higher = None
+        if self.veh.N_DER > 2:
+            R = plant_rows_der(self.vehicle.basis, self.T, t_rel, self.sample_time, n_samp)
+            R0, R1, higher = R[0], R[1], R[2:self.veh.N_DER]
+        else:
+            R0, R1 = plant_rows(self.vehicle.basis, self.T, t_rel, self.sample_time, n_samp)
         dist = None
         if self.disturbance is not None:
             filt, mean, stdev, scratch = self.disturbance
@@ -343,10 +592,13 @@ class BatchMPC(object):
         closed_loop_step(self.model, self.X, len(self.vehicle.basis), R0, R1, self.sample_time,
                          self.plant_x, self.plant_u,
                          (self.plant_x, self.plant_u, self.pred_x, self.pred_u), self.k, seed=self.seed,
-                         time_constant=self.time_constant, disturbance=dist)
+                         time_constant=self.time_constant, disturbance=dist, higher=higher)
         self.k += 1
         if self.ideal_prediction or self.ideal_update:
             self.veh.predict(self.X, t_rel, self.update_time, self.T, device=self.device_predict)
+        elif hasattr(self.veh, 'predict_planned'):
+            # signals other than state and input come from the planned trajectory (vehicle.py:326-328)
+            self.veh.predict_planned(self.X, t_rel, self.update_time, self.T, device=self.device_predict)
         if self.ideal_update:
             self.plant_x.copy_(self.torch.from_numpy(self.state))
             self.plant_u.copy_(self.torch.from_numpy(self.inp))

@@ -86,7 +86,7 @@ EXPORTS = ['omg_abi_version', 'omg_last_error', 'omg_default_options',
            'omg_admm_zl_update', 'omg_sample_batch', 'omg_tables_read',
            'omg_tables_free', 'omg_integrate_rk4', 'omg_feas_batch', 'omg_feas_batch_host',
            'omg_comm_unique_id', 'omg_comm_create', 'omg_comm_destroy', 'omg_admm_exchange_x',
-           'omg_admm_zl_update_dist', 'omg_closed_loop_step']
+           'omg_admm_zl_update_dist', 'omg_closed_loop_step', 'omg_closed_loop_step_der']
 
 _lib = None
 
@@ -143,6 +143,9 @@ def bind(lib):
     lib.omg_closed_loop_step.argtypes = ([C.c_int32] * 5 + [vp, C.c_int32, C.c_int32, vp, vp, C.c_double,
                                          C.c_int32, C.c_double, C.c_int32, C.c_int32, vp, vp, vp,
                                          C.c_uint64, C.c_int32] + [vp] * 8)
+    lib.omg_closed_loop_step_der.argtypes = ([C.c_int32] * 5 + [vp, C.c_int32, C.c_int32, C.c_int32, vp,
+                                             C.c_double, C.c_int32, C.c_double, C.c_int32, C.c_int32,
+                                             vp, vp, vp, C.c_uint64, C.c_int32] + [vp] * 8)
     lib.omg_tables_read.argtypes = [C.c_char_p]
     lib.omg_tables_read.restype = C.POINTER(_Tables)
     lib.omg_tables_free.argtypes = [C.POINTER(_Tables)]
@@ -658,7 +661,8 @@ def sample_batch(X, blocks, stream=None):
     return out
 
 
-ODE_MODELS = {'Holonomic': 0, 'Holonomic1D': 0, 'Holonomic3D': 0, 'Quadrotor3D': 1, 'Quadrotor': 2}
+ODE_MODELS = {'Holonomic': 0, 'Holonomic1D': 0, 'Holonomic3D': 0, 'Quadrotor3D': 1, 'Quadrotor': 2,
+              'Dubins': 3, 'HolonomicOrient': 4, 'SimpleQuadrotor3D': 5}
 
 
 def integrate_rk4(model, state0, inputs, sample_time, stream=None):
@@ -689,7 +693,7 @@ def disturbance_filter(fc):
 
 
 def closed_loop_step(model, X, L, R0, R1, sample_time, plant_x, plant_u, out, step, seed=0,
-                     time_constant=None, disturbance=None, stream=None):
+                     time_constant=None, disturbance=None, stream=None, higher=None):
     """Plant step of MPC step ``step`` for a batch (omg_closed_loop_step): the non-ideal
     simulate and predict of the reference's Vehicle from the plant state / last applied input
     (plant_x [B, n_state], plant_u [B, n_input]) along the trajectories of the spline
@@ -697,7 +701,10 @@ def closed_loop_step(model, X, L, R0, R1, sample_time, plant_x, plant_u, out, st
     out = (plant_x_next, plant_u_next, pred_x, pred_u), written in place (the plant outputs may
     be plant_x / plant_u themselves).  time_constant: first-order actuator lag (None = off).
     disturbance: (filt, mean, stdev, n_traj, scratch) with filt from disturbance_filter(fc) and
-    scratch a float64 tensor of at least B * n_input * (n_traj + 24) elements (None = off)."""
+    scratch a float64 tensor of at least B * n_input * (n_traj + 24) elements (None = off).
+    higher: the rows of derivatives 2 and 3 [k, n_samp+1, L] (divided by T^2, T^3), which the
+    quadrotor models read; with them, or for a model other than 0 and 1, the call goes to
+    omg_closed_loop_step_der."""
     lib = load_library()
     mid = ODE_MODELS[model] if isinstance(model, str) else int(model)
     tensors = (X, plant_x, plant_u) + tuple(out)
@@ -720,13 +727,24 @@ def closed_loop_step(model, X, L, R0, R1, sample_time, plant_x, plant_u, out, st
         if tuple(t.shape) != shape:
             raise ValueError('output tensor shapes do not match the plant state / input')
     d = disturbance is not None
-    rc = lib.omg_closed_loop_step(
-        mid, B, ns, ni, X.shape[1], X.data_ptr(), L, R0.shape[0] - 1, R0.ctypes.data, R1.ctypes.data,
-        float(sample_time), int(time_constant is not None),
-        float(time_constant) if time_constant is not None else 0., int(d), int(n_traj) if d else 0,
-        filt.ctypes.data if d else None, mean.ctypes.data if d else None,
-        stdev.ctypes.data if d else None, int(seed) & 0xFFFFFFFFFFFFFFFF, int(step),
-        plant_x.data_ptr(), plant_u.data_ptr(), *[t.data_ptr() for t in out],
-        scratch.data_ptr() if d else None, _stream_handle(on_gpu, X.device, stream))
+    rest = (float(sample_time), int(time_constant is not None),
+            float(time_constant) if time_constant is not None else 0., int(d), int(n_traj) if d else 0,
+            filt.ctypes.data if d else None, mean.ctypes.data if d else None,
+            stdev.ctypes.data if d else None, int(seed) & 0xFFFFFFFFFFFFFFFF, int(step),
+            plant_x.data_ptr(), plant_u.data_ptr(), *[t.data_ptr() for t in out],
+            scratch.data_ptr() if d else None, _stream_handle(on_gpu, X.device, stream))
+    if higher is None and mid in (0, 1):
+        rc = lib.omg_closed_loop_step(mid, B, ns, ni, X.shape[1], X.data_ptr(), L, R0.shape[0] - 1,
+                                      R0.ctypes.data, R1.ctypes.data, *rest)
+    else:
+        rows = [R0[None], R1[None]]
+        if higher is not None:
+            higher = np.asarray(higher, dtype=np.float64)
+            if higher.ndim != 3 or higher.shape[1:] != R0.shape:
+                raise ValueError('higher must be [k, n_samp + 1, L]')
+            rows.append(higher)
+        R = np.ascontiguousarray(np.concatenate(rows))
+        rc = lib.omg_closed_loop_step_der(mid, B, ns, ni, X.shape[1], X.data_ptr(), L, R0.shape[0] - 1,
+                                          R.shape[0], R.ctypes.data, *rest)
     if rc != 0:
         raise RuntimeError('libomgb200: %s' % lib.omg_last_error().decode())

@@ -1,11 +1,13 @@
 """Cost of closing the MPC loop through the vehicle dynamics (execution/batch_mpc.py).
 
-    python tools/closed_loop_bench.py [--batch 256] [--steps 50] [--runs 3] [--out DIR]
+    python tools/closed_loop_bench.py [--scenario config5] [--batch 256] [--steps 50] [--runs 3] [--out DIR]
 
-Config 5 (revolving door), B instances x N MPC steps, in two modes run alternately in one
-process: the ideal loop (the vehicle follows its spline) and the closed loop with the
-first-order actuator lag (tau = 0.1 s) and the filtered input disturbance (fc = 0.01,
-stdev = 0.05), the settings of the reference's p2p_holonomic_disturbances example.  Reported
+One scenario (default config 5, the revolving door), B instances x N MPC steps, in two modes
+run alternately in one process: the ideal loop (the vehicle follows its spline) and the closed
+loop with the first-order actuator lag (tau = 0.1 s) and the filtered input disturbance
+(fc = 0.01, stdev = 0.05 on every input), the settings of the reference's
+p2p_holonomic_disturbances example.  The update time is 0.1 s, 0.5 s for the Dubins
+scenarios (the steps of their recorded reference loops).  Reported
 per mode: the wall time per MPC step (a device synchronise closes every timed step), and in
 the closed loop the time of the plant-step launches alone from CUDA events around each call.
 The card's name and power limit are read in the same call.  Needs a CUDA device; prints one
@@ -22,8 +24,12 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-CLOSED = {'ideal_prediction': False, 'ideal_update': False, '1storder_delay': True, 'time_constant': 0.1,
-          'input_disturbance': {'fc': 0.01, 'stdev': 0.05 * np.ones(2)}}
+UPDATE_TIME = {'config_dubins_plain': 0.5, 'config_dubins': 0.5}
+
+
+def closed_options(n_input):
+    return {'ideal_prediction': False, 'ideal_update': False, '1storder_delay': True, 'time_constant': 0.1,
+            'input_disturbance': {'fc': 0.01, 'stdev': 0.05 * np.ones(n_input)}}
 
 
 def card():
@@ -32,15 +38,16 @@ def card():
     return q[0] if q else 'unknown'
 
 
-def one_run(mode, batch, steps):
+def one_run(mode, batch, steps, scenario='config5'):
     import torch
     from omg_tools_b200 import scenarios as sc
     from omg_tools_b200.execution.batch_mpc import BatchMPC
     from omg_tools_b200.solver import b200
-    pr = sc.config5()
+    pr = getattr(sc, scenario)()
     if mode == 'closed':
-        pr.vehicles[0].set_options(CLOSED)
-    bat = BatchMPC(pr, batch=batch, update_time=0.1, seed=1)
+        veh = pr.vehicles[0]
+        veh.set_options(closed_options(len(veh.prediction['input'])))
+    bat = BatchMPC(pr, batch=batch, update_time=UPDATE_TIME.get(scenario, 0.1), seed=1)
     plant_ms = []
     step_fn = b200.closed_loop_step
 
@@ -71,6 +78,7 @@ def one_run(mode, batch, steps):
 
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument('--scenario', default='config5', help='a function of omg_tools_b200.scenarios')
     ap.add_argument('--batch', type=int, default=256)
     ap.add_argument('--steps', type=int, default=50)
     ap.add_argument('--runs', type=int, default=3)
@@ -81,9 +89,11 @@ def main():
         raise SystemExit('closed_loop_bench.py needs a CUDA device')
     res = {'card': card(), 'device': torch.cuda.get_device_name(0), 'batch': a.batch, 'steps': a.steps,
            'ideal': [], 'closed': []}
+    if a.scenario != 'config5':
+        res['scenario'] = a.scenario
     for _ in range(a.runs):
         for mode in ('ideal', 'closed'):
-            res[mode].append(one_run(mode, a.batch, a.steps))
+            res[mode].append(one_run(mode, a.batch, a.steps, a.scenario))
     for mode in ('ideal', 'closed'):
         ms = [r['ms_per_step'] for r in res[mode]]
         res[mode + '_ms_per_step_median'] = float(np.median(ms))
@@ -92,7 +102,8 @@ def main():
     print(line)
     if a.out:
         os.makedirs(a.out, exist_ok=True)
-        with open(os.path.join(a.out, 'closed_loop_bench.json'), 'w') as f:
+        fname = 'closed_loop_bench.json' if a.scenario == 'config5' else 'closed_loop_bench_%s.json' % a.scenario
+        with open(os.path.join(a.out, fname), 'w') as f:
             f.write(line + '\n')
 
 
