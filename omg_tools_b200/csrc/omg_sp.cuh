@@ -147,26 +147,74 @@ __device__ __forceinline__ double sp_rcp(double x) { return __drcp_rn(x); }   //
 static inline double sp_rcp(double x) { return 1.0 / x; }
 #endif
 
-// term streams: SP_R independent 16-byte loads per chunk, then the sums in stream order.
-//   VAL(r) -> value of record r (uint4);  BODY uses o_ (the record's uint4) and acc_
-#define SP_STREAM16(ST, VAL, BODY)                                                           \
-  {                                                                                          \
-    const uint4* rp_ = reinterpret_cast<const uint4*>((ST).rec) + tid;                       \
-    double acc_ = 0.0;                                                                       \
-    for (int t_ = 0; t_ < (ST).n_chunk; ++t_, rp_ += SP_R * NT) {                            \
-      uint4 rr_[SP_R];                                                                       \
-      _Pragma("unroll")                                                                      \
-      for (int k_ = 0; k_ < SP_R; ++k_) rr_[k_] = __ldg(rp_ + k_ * NT);                      \
-      _Pragma("unroll")                                                                      \
-      for (int k_ = 0; k_ < SP_R; ++k_) {                                                    \
-        const uint4 o_ = rr_[k_];                                                            \
-        acc_ += (VAL);                                                                     \
-        if (o_.z & 0x8000u) { BODY acc_ = 0.0; }                                             \
-      }                                                                                      \
-    }                                                                                        \
+// out-of-line device code: one copy, outside the instruction range the iterations walk through
+#ifndef OMG_CPU_EMU
+#define SP_COLD __device__ __noinline__
+#define SP_HOT __device__ __noinline__
+#else
+#define SP_COLD static
+#define SP_HOT static inline
+static inline double __dmul_rn(double a, double b) { return a * b; }
+#endif
+
+#define SP_COEF(r) __hiloint2double((int)(r).y, (int)(r).x)
+
+// ---- thread streams: ONE out-of-line copy per record format -------------------------------
+// Every thread walks its own records, SP_R independent loads per chunk, and sums them in stream
+// order; the last record of an output carries an end flag.  The operands are offsets into sm, so
+// their loads stay shared-memory loads.
+//
+// 16-byte term records (PT16 {coef, cidx | end<<15, a, b, c}): out[c] (+)= the sum of
+// ((coef * V[cidx]) * P1[a]) * P2[b] over the output's records.  J points a at the 1.0 in
+// X[n] (x0 in b, the slot in c): ((coef * V) * 1.0) * X[x0] is what coef * V * X[x0] gives,
+// contracted or not.
+SP_HOT void sp_stream16(const SpStream st, const int v, const int p1, const int p2, double* out, const bool add) {
+  const int tid = threadIdx.x;
+  const uint4* rp = reinterpret_cast<const uint4*>(st.rec) + tid;
+  double acc = 0.0;
+  for (int t = 0; t < st.n_chunk; ++t, rp += SP_R * NT) {
+    uint4 rr[SP_R];
+#pragma unroll
+    for (int k = 0; k < SP_R; ++k) rr[k] = __ldg(rp + k * NT);
+#pragma unroll
+    for (int k = 0; k < SP_R; ++k) {
+      const uint4 o = rr[k];
+      acc += SP_COEF(o) * sm[v + (o.z & 0x7fffu)] * sm[p1 + (o.z >> 16)] * sm[p2 + (o.w & 0xffffu)];
+      if (o.z & 0x8000u) { const int c = (int)(o.w >> 16); out[c] = add ? out[c] + acc : acc; acc = 0.0; }
+    }
   }
-// 8-byte index streams; end flag = bit 16 of .y (bit 30 for H)
-#define SP_STREAM8(ST, ENDBIT, VAL, BODY)                                                    \
+}
+// 8-byte index records (x = i1 | i3<<16, y = i2 | dst<<16 | end<<30): t = the sum of
+// (P1[i1] * P2[i2 & mask]) * P3[i3] over the output's records.
+//   H (J^T Sigma J): P1 = P3 = jval, P2 = sg2 (i2 = row), out[dst] = t;
+//   C (J^T v by columns): P1 = jval, P2 = the 1.0 at xe[n] (mask 0, i2 = column), P3 = v,
+//     the value is the rhs entry -(gf[column] + t): out[dst] = it if out is given.
+// Returns the largest magnitude of the C values (0 for H).
+SP_HOT double sp_stream8(const SpStream st, const int p1, const int p2, const unsigned mask, const int p3,
+                         const int gfo, double* out) {
+  const int tid = threadIdx.x;
+  const uint2* rp = reinterpret_cast<const uint2*>(st.rec) + tid;
+  double acc = 0.0, mx = 0.0;
+  for (int t = 0; t < st.n_chunk; ++t, rp += SP_R * NT) {
+    uint2 rr[SP_R];
+#pragma unroll
+    for (int k = 0; k < SP_R; ++k) rr[k] = __ldg(rp + k * NT);
+#pragma unroll
+    for (int k = 0; k < SP_R; ++k) {
+      const uint2 o = rr[k];
+      acc += sm[p1 + (o.x & 0xffffu)] * sm[p2 + (o.y & mask)] * sm[p3 + (o.x >> 16)];
+      if (o.y & 0x40000000u) {
+        double val = acc;
+        if (gfo >= 0) { val = -(sm[gfo + (o.y & 0xffffu)] + acc); mx = fmax(mx, fabs(val)); }
+        if (out) out[(o.y >> 16) & 0x1fffu] = val;
+        acc = 0.0;
+      }
+    }
+  }
+  return mx;
+}
+// soft restoration (cold) runs the C stream on the trial vectors in the global scratch
+#define SP_STREAM8_GLOBAL(ST, JV, YV, BODY)                                                 \
   {                                                                                          \
     const uint2* rp_ = reinterpret_cast<const uint2*>((ST).rec) + tid;                       \
     double acc_ = 0.0;                                                                       \
@@ -177,25 +225,11 @@ static inline double sp_rcp(double x) { return 1.0 / x; }
       _Pragma("unroll")                                                                      \
       for (int k_ = 0; k_ < SP_R; ++k_) {                                                    \
         const uint2 o_ = rr_[k_];                                                            \
-        acc_ += (VAL);                                                                     \
-        if (o_.y & (ENDBIT)) { BODY acc_ = 0.0; }                                            \
+        acc_ += (JV)[o_.x & 0xffffu] * (YV)[o_.x >> 16];                                     \
+        if (o_.y & 0x40000000u) { BODY acc_ = 0.0; }                                         \
       }                                                                                      \
     }                                                                                        \
   }
-#define SP_COEF(r) __hiloint2double((int)(r).y, (int)(r).x)
-#define SP_VJ(X) (SP_COEF(o_) * V[o_.z & 0x7fffu] * (X)[o_.z >> 16])                       // J: a = x0, b = slot, c = row
-#define SP_VG(X) (SP_COEF(o_) * V[o_.z & 0x7fffu] * (X)[o_.z >> 16] * (X)[o_.w & 0xffffu])   // G: a, b = x0, x1, c = row
-#define SP_VC(JV, YV) ((JV)[o_.x & 0xffffu] * (YV)[o_.x >> 16])                             // C / R: slot | index<<16
-
-// out-of-line device code: one copy, outside the instruction range the iterations walk through
-#ifndef OMG_CPU_EMU
-#define SP_COLD __device__ __noinline__
-#define SP_HOT __device__ __noinline__
-#else
-#define SP_COLD static
-#define SP_HOT static inline
-static inline double __dmul_rn(double a, double b) { return a * b; }
-#endif
 
 // IEEE division, log and pow of the per-iteration passes: ONE out-of-line copy each instead of
 // an inlined expansion at every site (tens of call sites, each emitted once per unrolled copy).
@@ -316,24 +350,23 @@ __device__ __forceinline__ void sp_factor(const DevTab& T, const SpTab& P, const
       const int li = (e == 0xffffffffu) ? P.zslot : (int)(e & 0x1fffu);
       const int n4 = (int)d.z;
       double v0 = LK[li], v1 = 0.0;
-      uint4 r[4];
-      if (n4 > SP_NPF) {                                   // the rest of a long list: four loads in flight
-        const uint4* q_ = P.fpair + d.y + SP_NPF * 32;
+      // one loop body over the words in list order: the prefetched words first, then groups of
+      // four; the next group's four loads are in flight while the current one is summed
+      uint4 c[4];
 #pragma unroll
-        for (int t = 0; t < 4; ++t) if (SP_NPF + t < n4) r[t] = __ldg(q_ + t * 32);
-      }
-#pragma unroll
-      for (int w = 0; w < SP_NPF; ++w) if (n4 > w) SP_PAIR4(pA[w])
-      if (n4 > SP_NPF) {
-#pragma unroll
-        for (int t = 0; t < 4; ++t) if (SP_NPF + t < n4) SP_PAIR4(r[t])
-      }
-      for (int k = SP_NPF + 4; k < n4; k += 4) {
+      for (int t = 0; t < 4; ++t) c[t] = (t < SP_NPF) ? pA[t < SP_NPF ? t : 0] : make_uint4(0u, 0u, 0u, 0u);
+      int nc = (n4 < SP_NPF) ? n4 : SP_NPF;
+      uint4 r[4] = {};                   // words past the list are copied to c but never summed
+      for (int k = SP_NPF;; k += 4) {
         const uint4* q_ = P.fpair + d.y + k * 32;
 #pragma unroll
         for (int t = 0; t < 4; ++t) if (k + t < n4) r[t] = __ldg(q_ + t * 32);
 #pragma unroll
-        for (int t = 0; t < 4; ++t) if (k + t < n4) SP_PAIR4(r[t])
+        for (int t = 0; t < 4; ++t) if (t < nc) SP_PAIR4(c[t])
+        if (k >= n4) break;
+        nc = (n4 - k < 4) ? n4 - k : 4;
+#pragma unroll
+        for (int t = 0; t < 4; ++t) c[t] = r[t];
       }
       const double v = v0 + v1;
       if (e != 0xffffffffu) {
@@ -393,16 +426,14 @@ __device__ __forceinline__ void sp_factor(const DevTab& T, const SpTab& P, const
           } else {                                               // row q of the block: pivots, stores deferred
             const int c0 = (int)(tk.x & 0x7ffu);
             const unsigned eqb = (tk.x >> 17) & 15u;
-            if (q == 1) {
-              { const int jc = c0; SP_PIVOT(jc, d0, (eqb & 1u) != 0u) }
-              { const int jc = c0 + 1; SP_PIVOT(jc, d1, (eqb & 2u) != 0u) }
-              pv1 = d1; po1 = cb1;
-            } else if (q == 2) {
-              { const int jc = c0 + 2; SP_PIVOT(jc, d2, (eqb & 4u) != 0u) }
-              pv1 = a21; po1 = cb1 + 8; pv2 = d2; po2 = cb2;
-            } else {
-              { const int jc = c0 + 3; SP_PIVOT(jc, d3, (eqb & 8u) != 0u) }
-              pv1 = a31; po1 = cb1 + 16; pv2 = a32; po2 = cb2 + 8; pv3 = d3; po3 = cb3;
+            if (q == 1) { pv1 = d1; po1 = cb1; }
+            else if (q == 2) { pv1 = a21; po1 = cb1 + 8; pv2 = d2; po2 = cb2; }
+            else { pv1 = a31; po1 = cb1 + 16; pv2 = a32; po2 = cb2 + 8; pv3 = d3; po3 = cb3; }
+            // row q pivots column q (row 1 column 0 as well): one pivot expansion for all of them
+            for (int t = (q == 1) ? 0 : q; t <= q; ++t) {
+              const int jc = c0 + t;
+              const double dv = (t == 0) ? d0 : (t == 1) ? d1 : (t == 2) ? d2 : d3;
+              SP_PIVOT(jc, dv, ((eqb >> t) & 1u) != 0u)
             }
           }
         }
@@ -724,8 +755,9 @@ SP_COLD bool sp_setup(const DevTab& T, const SpTab& P, const omg_options& O, con
   const double smg = O.scaling_max_gradient;
   const double fsc = (fmaxv > smg) ? fmax(smg / fmaxv, 1e-8) : 1.0;
   // unscaled Jacobian -> jval, g -> gt
-  SP_STREAM16(P.J, SP_VJ(xe), jval[o_.w & 0xffffu] = acc_;)
-  SP_STREAM16(P.G, SP_VG(xe), gt[o_.w >> 16] = acc_;)
+  sp_stream16(P.J, S.V, S.xe, S.xe, jval, false);
+  sp_stream16(P.G, S.V, S.xe, S.xe, gt, false);
+  if (tid == 0) yd[m + 1] = fsc;         // the objective's multiplier in the W stream
   __syncthreads();
   for (int i = tid; i < m; i += NT) {
     const RowRec rr = T.rowrec[i];
@@ -803,7 +835,7 @@ SP_COLD bool sp_soft_resto(const DevTab& T, const SpTab& P, const omg_options& O
   const double* ubg = A.ubg + (A.bounds_shared ? 0 : (size_t)inst * m);
   const double rf = O.bound_relax_factor;
   __syncthreads();
-  SP_STREAM16(P.J, SP_VJ(xe), jval[o_.w & 0xffffu] = acc_;)      // (the factor is dead by now)
+  sp_stream16(P.J, S.V, S.xe, S.xe, jval, false);      // (the factor is dead by now)
   __syncthreads();
   double pv[1];
   pv[0] = 0.0;
@@ -816,7 +848,7 @@ SP_COLD bool sp_soft_resto(const DevTab& T, const SpTab& P, const omg_options& O
     if (r & 2) { zu = zU[i]; acc += fabs((sp_bound_up(ubg[i], dsc[i], rf) - si) * zu - mu); }
     pv[0] += acc + fabs(-y[i] - zl + zu);
   }
-  SP_STREAM8(P.C, 0x10000u, SP_VC(jval, yd), pv[0] += fabs(gf[o_.y & 0xffffu] + acc_);)
+  SP_STREAM8_GLOBAL(P.C, jval, yd, pv[0] += fabs(gf[o_.y & 0xffffu] + acc_);)
   block_reduce<OP_SUM>(pv, red);
   const double pd0 = pv[0];
   double alpha = a_p;
@@ -827,8 +859,8 @@ SP_COLD bool sp_soft_resto(const DevTab& T, const SpTab& P, const omg_options& O
     const double az = fmin(alpha, a_d);
     pv[0] = 0.0;
     // trial Jacobian -> jt (scratch), trial g -> gt, trial y -> wv
-    SP_STREAM16(P.J, SP_VJ(xt), jt[o_.w & 0xffffu] = acc_;)
-    SP_STREAM16(P.G, SP_VG(xt), gt[o_.w >> 16] = acc_;)
+    sp_stream16(P.J, S.V, S.xt, S.xt, jt, false);
+    sp_stream16(P.G, S.V, S.xt, S.xt, gt, false);
     __syncthreads();
     for (int i = tid; i < m; i += NT) {
       const int r = rt[i];
@@ -854,7 +886,7 @@ SP_COLD bool sp_soft_resto(const DevTab& T, const SpTab& P, const omg_options& O
       pv[0] += acc + fabs(-yt - zl + zu);
     }
     __syncthreads();
-    SP_STREAM8(P.C, 0x10000u, SP_VC(jt, wv),
+    SP_STREAM8_GLOBAL(P.C, jt, wv,
                { const int c_ = o_.y & 0xffffu;
                  pv[0] += fabs(ctl.fsc * sp_eval_range(T.DFt, T.dfptr[c_], T.dfptr[c_ + 1], V, xt) + acc_); })
     block_reduce<OP_SUM>(pv, red);
@@ -975,7 +1007,7 @@ __device__ __forceinline__ void ipm_body_sp(const DevTab& T, const SpTab& P, con
       rv[2] = 1e300;
       // ---- I1: Jacobian values (scaled) + per-row residual terms ---------------------
       // (loads by row type: a bound or multiplier that the row does not have is not fetched)
-      SP_STREAM16(P.J, SP_VJ(xe), jval[o_.w & 0xffffu] = acc_;)
+      sp_stream16(P.J, S.V, S.xe, S.xe, jval, false);
 #pragma unroll 1
       for (int i = tid; i < m; i += NT) {
         const int r = rt[i];
@@ -1004,7 +1036,7 @@ __device__ __forceinline__ void ipm_body_sp(const DevTab& T, const SpTab& P, con
       for (int j = tid; j < n; j += NT)
         gf[j] = ctl.fsc * sp_eval_range(T.DFt, T.dfptr[j], T.dfptr[j + 1], V, xe);
       __syncthreads();
-      SP_STREAM8(P.C, 0x10000u, SP_VC(jval, yd), rv[10] = fmax(rv[10], fabs(gf[o_.y & 0xffffu] + acc_));)
+      rv[10] = fmax(rv[10], sp_stream8(P.C, S.jval, S.xe + n, 0u, S.y, S.gf, nullptr));
       block_reduce<NRED_OPS>(rv, red);
       const double cinf = rv[0], maxprod = rv[1], minprod = rv[2], viol = rv[3];
       const double dinf = fmax(rv[10], rv[4]);
@@ -1079,19 +1111,13 @@ __device__ __forceinline__ void ipm_body_sp(const DevTab& T, const SpTab& P, con
       // inertia-correction retries.
       {
         // H positions: gather J^T Sigma J.  record: s1 | s2<<16, row | (dst | diag<<13 | end<<14)<<16
-        SP_STREAM8(P.H, 0x40000000u, jval[o_.x & 0xffffu] * sg2[o_.y & 0xffffu] * jval[o_.x >> 16],
-                   Kg[(o_.y >> 16) & 0x1fffu] = acc_;)
+        sp_stream8(P.H, S.jval, S.sig, 0xffffu, S.jval, -1, Kg);
         __syncthreads();
         TICK(5);
+        for (int i = tid; i < m; i += NT) sg2[i] = wv[i];   // sg2 is dead: w in shared memory for the rhs
         // Lagrangian Hessian W (lambda = y*dsc, objective factor fsc)
-        // record: a = lambda row (m: objective, m+1: padding), b = x0, c = L index
-        {
-          const double fsc_ = ctl.fsc;
-#define SP_LAM(lr) (((lr) < (unsigned)m) ? yd[lr] : (((lr) == (unsigned)m) ? fsc_ : 0.0))
-          SP_STREAM16(P.W, SP_COEF(o_) * V[o_.z & 0x7fffu] * SP_LAM(o_.z >> 16) * xe[o_.w & 0xffffu],
-                      Kg[o_.w >> 16] += acc_;)
-#undef SP_LAM
-        }
+        // record: a = lambda row (yd[m] = 0: padding, yd[m+1] = fsc: objective), b = x0, c = L index
+        sp_stream16(P.W, S.V, S.y, S.xe, Kg, true);
         // equality border + right-hand-side entries: one record per border slot
         // (slot | row<<16, L index; slot 0xffff: the rhs entry of the row)
         for (int e = tid; e < P.n_border; e += NT) {
@@ -1099,8 +1125,8 @@ __device__ __forceinline__ void ipm_body_sp(const DevTab& T, const SpTab& P, con
           const int i = (int)(b.x >> 16), sl = (int)(b.x & 0xffffu);
           Kg[b.y] = (sl == 0xffff) ? -(g[i] - __dmul_rn(lbg[i], dsc[i])) : dsc[i] * jval[sl];
         }
-        SP_STREAM8(P.C, 0x10000u, SP_VC(jval, wv),
-                   { Kg[(o_.y >> 17) & 0x1fffu] = -(gf[o_.y & 0xffffu] + acc_); })
+        __syncthreads();
+        sp_stream8(P.C, S.jval, S.xe + n, 0u, S.sig, S.gf, Kg);
         sp_fence_async();                    // Kg reaches L2 (the fence carries MEMBAR.ALL.GPU) and is
         __syncthreads();                     // ordered before the async-proxy read; no L1 invalidation
       }
@@ -1155,7 +1181,7 @@ __device__ __forceinline__ void ipm_body_sp(const DevTab& T, const SpTab& P, con
       // J dx through the row ELL -> ds (temporarily)
       // (the Jacobian values were overwritten by the factor: J dx straight from the terms;
       //  record: a = x0, b = column, c = row)
-      SP_STREAM16(P.R, SP_COEF(o_) * V[o_.z & 0x7fffu] * xe[o_.z >> 16] * dx[o_.w & 0xffffu], ds[o_.w >> 16] = acc_;)
+      sp_stream16(P.R, S.V, S.xe, S.dx, ds, false);
       __syncthreads();
 #pragma unroll 1
       for (int i = tid; i < m; i += NT) {
@@ -1199,7 +1225,7 @@ __device__ __forceinline__ void ipm_body_sp(const DevTab& T, const SpTab& P, con
         for (int j = tid; j < n; j += NT) xt[j] = xe[j] + alpha * dx[j];
         if (tid == 0) xt[n] = 1.0;
         __syncthreads();
-        SP_STREAM16(P.G, SP_VG(xt), gt[o_.w >> 16] = acc_;)
+        sp_stream16(P.G, S.V, S.xt, S.xt, gt, false);
         __syncthreads();
         double tv[3];
         tv[0] = 0.0; tv[1] = 0.0; tv[2] = 0.0;

@@ -512,14 +512,14 @@ static bool sp_setup(omg_problem* h, const omg_tables* tb, const cudaDeviceProp&
   auto xi_of = [&](const omg_termlist& L, int t, int w) { return (w < L.width) ? L.xi[(size_t)t * L.width + w] : n; };
   auto end16 = [](PT16& r) { r.cidx |= 0x8000u; };
   PT16 pad16; pad16.coef = 0.0; pad16.cidx = 0; pad16.a = (unsigned short)n; pad16.b = (unsigned short)n; pad16.c = 0;
-  {  // J: a = x0, b = slot, c = row
+  {  // J: a = n (x[n] = 1.0), b = x0, c = slot
     std::vector<std::vector<PT16>> lists(tb->nnz_j);
     std::vector<PT16> dum(tb->nnz_j);
     for (int s = 0; s < tb->nnz_j; ++s) {
-      PT16 d = pad16; d.b = (unsigned short)s; d.c = (unsigned short)tb->jrow[s]; dum[s] = d;
+      PT16 d = pad16; d.c = (unsigned short)s; dum[s] = d;
       for (int t = tb->J.ptr[s]; t < tb->J.ptr[s + 1]; ++t) {
         PT16 r; r.coef = tb->J.coef[t]; r.cidx = (unsigned short)tb->J.cidx[t];
-        r.a = (unsigned short)xi_of(tb->J, t, 0); r.b = (unsigned short)s; r.c = (unsigned short)tb->jrow[s];
+        r.a = (unsigned short)n; r.b = (unsigned short)xi_of(tb->J, t, 0); r.c = (unsigned short)s;
         lists[s].push_back(r);
       }
     }
@@ -542,8 +542,8 @@ static bool sp_setup(omg_problem* h, const omg_tables* tb, const cudaDeviceProp&
     sp_build_stream(lists, dum, pad16, end16, nt, out, &P.G.n_chunk);
     P.G.rec = upload(h, out.data(), out.size(), &ok);
   }
-  {  // W: a = lambda row, b = x0, c = L index
-    PT16 padw = pad16; padw.a = (unsigned short)(m + 1); padw.c = (unsigned short)P.zslot;
+  {  // W: a = lambda row (m: padding, y[m] = 0; m + 1: the objective, y[m+1] = its factor), b = x0, c = L index
+    PT16 padw = pad16; padw.a = (unsigned short)m; padw.c = (unsigned short)P.zslot;
     std::vector<std::vector<PT16>> lists(tb->nnz_w);
     std::vector<PT16> dum(tb->nnz_w, padw);
     for (int q = 0; q < tb->nnz_w; ++q) {
@@ -551,7 +551,8 @@ static bool sp_setup(omg_problem* h, const omg_tables* tb, const cudaDeviceProp&
       dum[q].c = (unsigned short)dst;
       for (int t = tb->W.ptr[q]; t < tb->W.ptr[q + 1]; ++t) {
         PT16 r; r.coef = tb->W.coef[t]; r.cidx = (unsigned short)tb->W.cidx[t];
-        r.a = (unsigned short)(tb->W.lrow ? tb->W.lrow[t] : m); r.b = (unsigned short)xi_of(tb->W, t, 0);
+        const int lr = tb->W.lrow ? tb->W.lrow[t] : m;
+        r.a = (unsigned short)((lr == m) ? m + 1 : lr); r.b = (unsigned short)xi_of(tb->W, t, 0);
         r.c = (unsigned short)dst;
         lists[q].push_back(r);
       }
@@ -577,14 +578,14 @@ static bool sp_setup(omg_problem* h, const omg_tables* tb, const cudaDeviceProp&
                     [](uint2& r) { r.y |= 0x40000000u; }, nt, out, &P.H.n_chunk);
     P.H.rec = upload(h, out.data(), out.size(), &ok);
   }
-  {  // C (columns: J^T v): x = slot | row<<16, y = column | end<<16 | rhs L index<<17
+  {  // C (columns: J^T v): x = slot | row<<16, y = column | rhs L index<<16 | end<<30
     std::vector<std::vector<uint2>> cl(n);
     std::vector<uint2> cd(n);
-    auto ctag = [&](int j) { return (unsigned)j | ((unsigned)rhsidx[Y.pos[j]] << 17); };
+    auto ctag = [&](int j) { return (unsigned)j | ((unsigned)rhsidx[Y.pos[j]] << 16); };
     for (int j = 0; j < n; ++j) cd[j] = make_uint2((unsigned)m << 16, ctag(j));
     for (int s = 0; s < tb->nnz_j; ++s)
       cl[tb->jcol[s]].push_back(make_uint2((unsigned)s | ((unsigned)tb->jrow[s] << 16), ctag(tb->jcol[s])));
-    auto end8 = [](uint2& r) { r.y |= 0x10000u; };
+    auto end8 = [](uint2& r) { r.y |= 0x40000000u; };
     std::vector<uint2> out;
     sp_build_stream(cl, cd, make_uint2((unsigned)m << 16, 0u), end8, nt, out, &P.C.n_chunk);
     P.C.rec = upload(h, out.data(), out.size(), &ok);

@@ -140,7 +140,8 @@ def footprint(csrc=CSRC):
     for _, op, chain, _ in rng:
         ln = line(chain)
         per[next((PHASES[k] for k, (p, q) in prng.items() if ln and p <= ln <= q), 'other')] += 16
-    callees = sorted({m for _, op, _, _ in rng for m in re.findall(r'CALL\.\S+ `\((\S+?)\)', op)})
+    calls = collections.Counter(m for _, op, _, _ in rng for m in re.findall(r'CALL\.\S+ `\((\S+?)\)', op))
+    callees = sorted(calls)
     return {
         'kernel_bytes': 16 * len(ins),
         'range_bytes': 16 * len(rng),
@@ -149,6 +150,7 @@ def footprint(csrc=CSRC):
         'stl': sum(1 for e in rng if re.match(r'(@\S+\s+)?STL\b', e[1])),
         'ldl': sum(1 for e in rng if re.match(r'(@\S+\s+)?LDL\b', e[1])),
         'callees': {c: sub.get(c, 0) for c in callees},
+        'calls': calls,                  # call sites in the range per out-of-line function
         'ptxas': rep.get(KERNEL, {}),
         'others': {k: 16 * sum(1 for e in v if e[0] is not None)
                    for k, v in secs.items() if 'omg_ipm_kernel' in k and k != KERNEL},
@@ -164,9 +166,9 @@ def main():
           % (r['range_bytes'], r['range_start'], r['range_end'], r['stl'], r['ldl']))
     for name in list(PHASES.values()) + ['other']:
         print('  %-22s %8d' % (name, r['phases'].get(name, 0)))
-    print('out-of-line functions called from the range (bytes):')
+    print('out-of-line functions called from the range (bytes, call sites):')
     for c, s in r['callees'].items():
-        print('  %-60s %8d' % (c.split('$')[-1], s))
+        print('  %-60s %8d %4d' % (c.split('$')[-1], s, r['calls'][c]))
     print('other kernels (bytes of SASS):')
     for k, s in sorted(r['others'].items()):
         print('  %-60s %8d' % (k, s))
