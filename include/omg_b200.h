@@ -246,6 +246,49 @@ int omg_sample_batch(int32_t B, int32_t n, const double* x, int32_t n_blocks,
                      const int32_t* offs, const int32_t* lens, const int32_t* ncols,
                      const int32_t* nsamp, const double* S, double* out, void* stream);
 
+/* Per-instance spline bases (free motion time, where every instance has its own T and so its own
+ * abscissae).  The spline variables are given as n_blocks blocks (HOST int arrays offs, lens, ncols,
+ * degrees [n_blocks]: offset in x, basis length L, columns, degree p; HOST knots: the L + p + 1
+ * knots of each block, concatenated), column c of block k at x[b, offs[k] + c * L ..].  Bounds of
+ * both calls: 0 <= p <= OMG_SPL_MAX_DEGREE and p + 1 <= L <= OMG_SPL_MAX_LEN.  Basis values follow
+ * BSplineBasis.eval_basis (reference spline.py:131-136, 214-233): Cox-de Boor, the leading clamped
+ * intervals closed on both ends, every other interval (k_i, k_i+1], zero-length spans skipped.
+ * Descriptors are uploaded by the call, which copies the host arrays before it returns.
+ * Asynchronous on `stream`. */
+#define OMG_SPL_MAX_DEGREE 8
+#define OMG_SPL_MAX_LEN 48
+
+/* Free-T warm start, the per-instance counterpart of omg_shift_batch (reference
+ * FreeTPoint2point.init_step, point2point.py:354-368, with shift_spline, spline_extra.py:88-99,
+ * and BSplineBasis.transform, spline.py:280-306).  For every instance b with active[b] != 0
+ * (active: DEVICE int32 [B], or NULL for all): T = x[b, t_index]; u = T - update_time and
+ * target = T if T < 2 update_time, else u = update_time and target = T - update_time;
+ * tau = u / target.  Each block is re-expressed on the basis with knots [tau] * p +
+ * linspace(tau, end, L - p + 1) + [end] * p (end: the block's last knot), collocated at the first
+ * arg-max of each new basis function over linspace(tau, end, 501); the transformation's entries
+ * below 1e-10 are dropped.  Then x[b, t_index] = target.  Instances with tau outside (0, 1) are
+ * left alone.  x: DEVICE [B][n] with n the problem's, in place.  Rejected with a message:
+ * update_time <= 0, t_index outside [0, n), null pointers, blocks outside x, and degrees or
+ * lengths beyond the bounds above. */
+int omg_shift_free_batch(omg_problem* h, int32_t B, double* x, int32_t t_index, double update_time,
+                         const int32_t* active, int32_t n_blocks, const int32_t* offs,
+                         const int32_t* lens, const int32_t* ncols, const int32_t* degrees,
+                         const double* knots, void* stream);
+
+/* Per-instance spline evaluation, the counterpart of omg_sample_batch for abscissae that differ
+ * between instances (reference Vehicle.store -> splines2signals at t / T, vehicle.py:250-300):
+ * out[b] = concat over blocks of [column][point][derivative], the d-th derivative (d < n_der) of
+ * the column at tau[b][j] divided by scale[b]^d.  Derivatives as BSplineBasis.derivative
+ * (spline.py:236-260).  DEVICE x [B][n], tau [B][n_pts], scale [B], out
+ * [B][sum ncols * n_pts * n_der].  Any finite tau is valid (outside the knot span every value is
+ * 0): callers pad their point sets with such points.  Rejected with a message: n_der outside
+ * 1 .. 4 or above p + 1 of a block, n_pts < 1, null pointers, blocks outside x, degrees or lengths
+ * beyond the bounds above, and more than 48 KB of derivative coefficients per instance. */
+int omg_eval_batch(int32_t B, int32_t n, const double* x, int32_t n_blocks, const int32_t* offs,
+                   const int32_t* lens, const int32_t* ncols, const int32_t* degrees,
+                   const double* knots, int32_t n_pts, const double* tau, const double* scale,
+                   int32_t n_der, double* out, void* stream);
+
 /* Non-ideal state prediction for a batch (DEVICE pointers): integrate the vehicle ODE from
  * state0 [B x n_state] over `steps` samples of the planned input trajectory
  * inputs [B x (steps+1) x n_input] with classical RK4, result in stateT [B x n_state].

@@ -1529,6 +1529,212 @@ __global__ void omg_sample_kernel(const double* __restrict__ x, int B, int n, in
 }
 
 // ---------------------------------------------------------------------------
+// Per-instance spline bases (free motion time: every instance has its own tau = dt / T_b, so no
+// basis row can be shared across the batch).  Block descriptors are 6 ints per spline variable:
+// {offset in x, basis length L, columns, degree p, offset of its L + p + 1 knots, offset of its
+// derivative coefficients in shared memory (omg_eval_kernel)}.
+// ---------------------------------------------------------------------------
+#ifdef OMG_CPU_EMU
+static inline double __dadd_rn(double a, double b) { return a + b; }   // (__dmul_rn: omg_sp.cuh)
+#endif
+#define OMG_SPL_DESC 6
+#define OMG_SPL_GRID 501      // NO_POINTS of basics/spline.py: the collocation grid
+#define OMG_SPL_DROP 1e-10    // _DROP_TOL of basics/spline.py
+
+// Cox-de Boor recursion of BSplineBasis.eval_basis (basics/spline.py; reference spline.py:131-136,
+// 214-233) for the basis functions i0 .. i0+cnt-1 of degree p on the knots k: w holds cnt + p
+// doubles, the values end in w[0..cnt).  The leading clamped intervals (i < p + 1 and k[i] == k[0])
+// are closed on both ends, every other interval is (k_i, k_i+1]; zero-length spans are skipped
+// (den == 0).  Each value is rounded in the order numpy rounds it (no contraction into an FMA), so
+// the values are the host's bit for bit: the collocation points of omg_shift_free_kernel are
+// arg-max positions and depend on ties between them.
+__device__ void omg_cox_de_boor(const double* k, int p, double x, int i0, int cnt, double* w) {
+  for (int j = 0; j < cnt + p; ++j) {
+    const int i = i0 + j;
+    const bool closed = i < p + 1 && k[0] == k[i];
+    w[j] = ((closed ? x >= k[i] : x > k[i]) && x <= k[i + 1]) ? 1.0 : 0.0;
+  }
+  for (int d = 1; d <= p; ++d)
+    for (int j = 0; j < cnt + p - d; ++j) {      // (w[j + 1] is still the previous degree's)
+      const int i = i0 + j;
+      double acc = 0.0, den = k[i + d] - k[i];
+      if (den != 0.0) acc = __dadd_rn(acc, __dmul_rn(x - k[i], w[j]) / den);
+      den = k[i + d + 1] - k[i + 1];
+      if (den != 0.0) acc = __dadd_rn(acc, __dmul_rn(k[i + d + 1] - x, w[j + 1]) / den);
+      w[j] = acc;
+    }
+}
+
+// numpy.linspace(a, b, num)[i]: i * ((b - a) / (num - 1)) + a, and b itself at the end
+__device__ __forceinline__ double omg_linspace(double a, double b, int num, int i) {
+  return i == num - 1 ? b : __dadd_rn(__dmul_rn((double)i, (b - a) / (double)(num - 1)), a);
+}
+
+// Free-T warm start of one instance per block (reference FreeTPoint2point.init_step,
+// point2point.py:354-368, with shift_spline, spline_extra.py:88-99): from T = x[t_index] the
+// update u and target time (u = T - dt, target = T when T < 2 dt; else u = dt, target = T - dt),
+// tau = u / target; every block is re-expressed on shift_spline's basis
+//   knots2 = [tau] * p + linspace(tau, end, L - p + 1) + [end] * p
+// by BSplineBasis.transform: collocation at the first arg-max of each new basis function over
+// linspace(tau, end, 501), M = bm^-1 old_basis(points), entries below 1e-10 dropped, c <- M c.
+// Then x[t_index] = target.  Inactive instances and tau outside (0, 1) are left alone.
+// Shared memory: x row [n] | knots2 [Lmax + pmax + 1] | points [Lmax] | arg-max scratch
+// [2 blockDim] | bm [Lmax^2] | old_basis(points), then M [Lmax^2].
+__global__ void omg_shift_free_kernel(double* x, int B, int n, int t_index, double dt,
+                                      const int* __restrict__ active, int n_blocks,
+                                      const int* __restrict__ desc, const double* __restrict__ kn,
+                                      int Lmax, int pmax) {
+  OMG_DYN_SHARED(xs);
+  const int b = blockIdx.x, t = threadIdx.x, nt = blockDim.x;
+  if (b >= B || (active && !active[b])) return;
+  double* xb = x + (size_t)b * n;
+  const double T = xb[t_index];
+  double u = dt, target = T - dt;
+  if (T < 2.0 * dt) { u = T - dt; target = T; }
+  const double tau = u / target;
+  if (!(tau > 0.0 && tau < 1.0)) return;
+  double* k2 = xs + n;
+  double* xm = k2 + Lmax + pmax + 1;
+  double* sv = xm + Lmax;
+  double* sg = sv + nt;
+  double* A = sg + nt;
+  double* R = A + (size_t)Lmax * Lmax;
+  for (int i = t; i < n; i += nt) xs[i] = xb[i];
+  for (int blk = 0; blk < n_blocks; ++blk) {
+    const int* dsc = desc + OMG_SPL_DESC * blk;
+    const int off = dsc[0], L = dsc[1], nc = dsc[2], p = dsc[3];
+    const double* ko = kn + dsc[4];
+    const double end = ko[L + p];
+    const int nk = L - p + 1;
+    __syncthreads();                              // (x row loaded / previous block done)
+    for (int j = t; j < L + p + 1; j += nt)
+      k2[j] = j < p ? tau : (j < p + nk ? omg_linspace(tau, end, nk, j - p) : end);
+    __syncthreads();
+    // collocation points: S segments of the grid per basis function, the first maximum of each
+    // segment, then the first maximum over the segments in grid order (numpy.argmax)
+    const int S = nt / L > 0 ? nt / L : 1, seg = (OMG_SPL_GRID + S - 1) / S;
+    if (t < L * S) {
+      const int l = t % L, s = t / L;
+      double w[OMG_SPL_MAX_DEGREE + 1], best = -1.0;
+      int bg = -1;
+      const int g1 = min(OMG_SPL_GRID, (s + 1) * seg);
+      for (int g = s * seg; g < g1; ++g) {
+        const double xg = omg_linspace(tau, end, OMG_SPL_GRID, g);
+        double v = 0.0;                           // (exactly 0 outside the support)
+        if (xg >= k2[l] && xg <= k2[l + p + 1]) { omg_cox_de_boor(k2, p, xg, l, 1, w); v = w[0]; }
+        if (v > best) { best = v; bg = g; }
+      }
+      sv[t] = best; sg[t] = (double)bg;
+    }
+    __syncthreads();
+    for (int l = t; l < L; l += nt) {
+      double best = -1.0; int bg = 0;
+      for (int s = 0; s < S; ++s)
+        if (sg[s * L + l] >= 0.0 && sv[s * L + l] > best) { best = sv[s * L + l]; bg = (int)sg[s * L + l]; }
+      xm[l] = omg_linspace(tau, end, OMG_SPL_GRID, bg);
+    }
+    __syncthreads();
+    // bm = new_basis(points), R = old_basis(points)
+    for (int i = t; i < L; i += nt) {
+      double w[OMG_SPL_MAX_LEN + OMG_SPL_MAX_DEGREE];
+      omg_cox_de_boor(k2, p, xm[i], 0, L, w);
+      for (int l = 0; l < L; ++l) A[i * L + l] = w[l];
+      omg_cox_de_boor(ko, p, xm[i], 0, L, w);
+      for (int l = 0; l < L; ++l) R[i * L + l] = w[l];
+    }
+    // bm M = R by Gaussian elimination WITHOUT pivoting: a collocation matrix of a B-spline basis
+    // at points that satisfy Schoenberg-Whitney (each point inside its function's support) is
+    // banded and totally positive, and for such matrices elimination without pivoting is stable
+    // (de Boor & Pinkus 1977).  The host's LU with partial pivoting rounds differently.
+    for (int j = 0; j < L - 1; ++j) {
+      __syncthreads();
+      const double piv = A[j * L + j];
+      const int nr = L - 1 - j, wa = L - 1 - j, wr = wa + L;
+      for (int e = t; e < nr * wr; e += nt) {
+        const int i = j + 1 + e / wr, c = e % wr;
+        const double f = A[i * L + j] / piv;
+        if (c < wa) A[i * L + j + 1 + c] -= f * A[j * L + j + 1 + c];
+        else R[i * L + c - wa] -= f * R[j * L + c - wa];
+      }
+    }
+    __syncthreads();
+    for (int c = t; c < L; c += nt)
+      for (int i = L - 1; i >= 0; --i) {
+        double s = R[i * L + c];
+        for (int k = i + 1; k < L; ++k) s -= A[i * L + k] * R[k * L + c];
+        R[i * L + c] = s / A[i * L + i];
+      }
+    __syncthreads();
+    for (int e = t; e < L * nc; e += nt) {
+      const int c = e / L, i = e - c * L;
+      double acc = 0.0;
+      for (int k = 0; k < L; ++k) {
+        const double m = R[i * L + k];
+        if (fabs(m) >= OMG_SPL_DROP) acc += m * xs[off + c * L + k];
+      }
+      xb[off + c * L + i] = acc;
+    }
+  }
+  __syncthreads();                                // (every thread has read T)
+  if (t == 0) xb[t_index] = target;
+}
+
+// Per-instance evaluation, one instance per block: out[b, blk, c, j, d] = d-th derivative of
+// column c of block blk at tau[b, j], divided by scale[b]^d (d < n_der).  Derivatives as
+// BSplineBasis.derivative takes them (de Boor X.16): coefficients c' = (p - i) (c_j+1 - c_j) /
+// (k_j+p+1 - k_j+i+1) per order i on the basis of degree p - d and knots k[d : -d]; a span of
+// zero length gives a zero coefficient (its basis function vanishes).
+__global__ void omg_eval_kernel(const double* __restrict__ x, int B, int n, int n_blocks,
+                                const int* __restrict__ desc, const double* __restrict__ kn, int n_pts,
+                                const double* __restrict__ tau, const double* __restrict__ scale,
+                                int n_der, double* __restrict__ out, int n_out) {
+  OMG_DYN_SHARED(cd);                       // per block and column: n_der rows of L coefficients
+  const int b = blockIdx.x, t = threadIdx.x, nt = blockDim.x;
+  if (b >= B) return;
+  const double* xb = x + (size_t)b * n;
+  int n_col = 0;
+  for (int blk = 0; blk < n_blocks; ++blk) n_col += desc[OMG_SPL_DESC * blk + 2];
+  for (int e = t; e < n_col; e += nt) {
+    int blk = 0, c = e;
+    while (c >= desc[OMG_SPL_DESC * blk + 2]) c -= desc[OMG_SPL_DESC * blk++ + 2];
+    const int* dsc = desc + OMG_SPL_DESC * blk;
+    const int L = dsc[1], p = dsc[3];
+    const double* k = kn + dsc[4];
+    double* q = cd + dsc[5] + (size_t)c * n_der * L;
+    for (int i = 0; i < L; ++i) q[i] = xb[dsc[0] + c * L + i];
+    for (int d = 1; d < n_der; ++d)
+      for (int j = 0; j < L - d; ++j) {
+        const double den = k[j + p + 1] - k[j + d];
+        q[d * L + j] = den != 0.0 ? (p - d + 1) * (q[(d - 1) * L + j + 1] - q[(d - 1) * L + j]) / den : 0.0;
+      }
+  }
+  __syncthreads();
+  const double s = scale[b];
+  double* ob = out + (size_t)b * n_out;
+  int ooff = 0;
+  for (int blk = 0; blk < n_blocks; ++blk) {
+    const int* dsc = desc + OMG_SPL_DESC * blk;
+    const int L = dsc[1], nc = dsc[2], p = dsc[3];
+    const double* k = kn + dsc[4];
+    for (int j = t; j < n_pts; j += nt) {
+      const double xj = tau[(size_t)b * n_pts + j];
+      double w[OMG_SPL_MAX_LEN + OMG_SPL_MAX_DEGREE], sd = 1.0;
+      for (int d = 0; d < n_der; ++d) {
+        omg_cox_de_boor(k + d, p - d, xj, 0, L - d, w);
+        for (int c = 0; c < nc; ++c) {
+          const double* q = cd + dsc[5] + ((size_t)c * n_der + d) * L;
+          double acc = 0.0;
+          for (int i = 0; i < L - d; ++i) acc += w[i] * q[i];
+          ob[ooff + ((size_t)c * n_pts + j) * n_der + d] = acc / sd;
+        }
+        sd *= s;
+      }
+    }
+    ooff += nc * n_pts * n_der;
+  }
+}
+
+// ---------------------------------------------------------------------------
 // ADMM consensus step of one agent per block (reference admm.py:117-168 z-update,
 // 248-266 lambda-update, 268-307 residuals), in first-knot-shifted coordinates:
 //   v   = Tf (x + l/rho)            for the own copy and every neighbour copy
@@ -2505,6 +2711,95 @@ int omg_sample_batch(int32_t B, int32_t n, const double* x, int32_t n_blocks, co
   OMG_LAUNCH(omg_sample_kernel, B, 128, sizeof(double) * n, stream, x, B, n, n_blocks, d_i, d_i + n_blocks, d_i + 2 * n_blocks,
                                                            d_i + 3 * n_blocks, d_i + 4 * n_blocks, d_i + 5 * n_blocks,
                                                            cache.d_d, out, otot);
+  CK(cudaGetLastError());
+  return 0;
+}
+
+// Descriptors of omg_shift_free_batch / omg_eval_batch (OMG_SPL_DESC ints per block, see
+// omg_shift_free_kernel); false with a message naming `fn` when a block is out of bounds.  n_der
+// rows of derivative coefficients per column are counted into *n_coef.
+static bool spline_desc(const std::string& fn, int32_t n, int32_t n_blocks, const int32_t* offs,
+                        const int32_t* lens, const int32_t* ncols, const int32_t* degrees,
+                        const double* knots, int n_der, std::vector<int>& iv, size_t* n_knots,
+                        int* Lmax, int* pmax, size_t* n_coef) {
+  iv.assign((size_t)OMG_SPL_DESC * n_blocks, 0);
+  *n_knots = 0; *n_coef = 0; *Lmax = 1; *pmax = 0;
+  for (int k = 0; k < n_blocks; ++k) {
+    const int L = lens[k], p = degrees[k], nc = ncols[k], off = offs[k];
+    const std::string blk = fn + ": block " + std::to_string(k) + ": ";
+    if (p < 0 || p > OMG_SPL_MAX_DEGREE || L < p + 1 || L > OMG_SPL_MAX_LEN) {
+      set_err(blk + "degree " + std::to_string(p) + " / basis length " + std::to_string(L) + " outside 0 <= p <= " +
+              std::to_string(OMG_SPL_MAX_DEGREE) + ", p + 1 <= L <= " + std::to_string(OMG_SPL_MAX_LEN));
+      return false;
+    }
+    if (nc < 1 || off < 0 || (int64_t)off + (int64_t)L * nc > n) { set_err(blk + "columns outside x"); return false; }
+    if (n_der > p + 1) {
+      set_err(blk + "n_der " + std::to_string(n_der) + " above degree + 1 = " + std::to_string(p + 1)); return false; }
+    const double* kk = knots + *n_knots;
+    for (int j = 0; j < L + p; ++j)
+      if (!(kk[j] <= kk[j + 1])) { set_err(blk + "knots not non-decreasing"); return false; }
+    int* d = iv.data() + (size_t)OMG_SPL_DESC * k;
+    d[0] = off; d[1] = L; d[2] = nc; d[3] = p; d[4] = (int)*n_knots; d[5] = (int)*n_coef;
+    *n_knots += L + p + 1;
+    *n_coef += (size_t)nc * n_der * L;
+    *Lmax = std::max(*Lmax, L); *pmax = std::max(*pmax, p);
+  }
+  return true;
+}
+
+int omg_shift_free_batch(omg_problem* h, int32_t B, double* x, int32_t t_index, double update_time,
+                         const int32_t* active, int32_t n_blocks, const int32_t* offs, const int32_t* lens,
+                         const int32_t* ncols, const int32_t* degrees, const double* knots, void* stream_) {
+  const std::string f("omg_shift_free_batch");
+  if (!h || !x || n_blocks < 0 || (n_blocks > 0 && (!offs || !lens || !ncols || !degrees || !knots))) {
+    set_err(f + ": null argument"); return -1; }
+  if (!(update_time > 0.0)) { set_err(f + ": update_time must be > 0"); return -1; }
+  if (t_index < 0 || t_index >= h->T.n) {
+    set_err(f + ": t_index " + std::to_string(t_index) + " outside [0, " + std::to_string(h->T.n) + ")"); return -1; }
+  std::vector<int> iv;
+  size_t nk = 0, nco = 0;
+  int Lmax = 1, pmax = 0;
+  if (!spline_desc(f, h->T.n, n_blocks, offs, lens, ncols, degrees, knots, 1, iv, &nk, &Lmax, &pmax, &nco)) return -1;
+  if (B <= 0) return 0;
+  const int nt = 128;
+  const size_t smem = sizeof(double) * ((size_t)h->T.n + 2 * (size_t)Lmax + pmax + 1 + 2 * nt + 2 * (size_t)Lmax * Lmax);
+  if (smem > 227 * 1024) { set_err(f + ": x row and bases exceed the shared memory of a block"); return -1; }
+  cudaStream_t stream = (cudaStream_t)stream_;
+  CK(cudaSetDevice(h->device));
+  static thread_local DescCache cache;         // (one descriptor per host thread, as omg_sample_batch)
+  if (desc_upload(cache, h->device, iv, knots, nk, stream)) return -1;
+  if (smem > 48 * 1024)
+    CK(cudaFuncSetAttribute((const void*)omg_shift_free_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  OMG_LAUNCH(omg_shift_free_kernel, B, nt, smem, stream, x, B, h->T.n, t_index, update_time, active, n_blocks,
+             cache.d_i, cache.d_d, Lmax, pmax);
+  CK(cudaGetLastError());
+  return 0;
+}
+
+int omg_eval_batch(int32_t B, int32_t n, const double* x, int32_t n_blocks, const int32_t* offs,
+                   const int32_t* lens, const int32_t* ncols, const int32_t* degrees, const double* knots,
+                   int32_t n_pts, const double* tau, const double* scale, int32_t n_der, double* out,
+                   void* stream_) {
+  const std::string f("omg_eval_batch");
+  if (!x || !tau || !scale || !out || n_blocks < 0 ||
+      (n_blocks > 0 && (!offs || !lens || !ncols || !degrees || !knots))) { set_err(f + ": null argument"); return -1; }
+  if (n_der < 1 || n_der > 4) { set_err(f + ": n_der " + std::to_string(n_der) + " outside 1 .. 4"); return -1; }
+  if (n_pts < 1) { set_err(f + ": n_pts must be >= 1"); return -1; }
+  std::vector<int> iv;
+  size_t nk = 0, nco = 0;
+  int Lmax = 1, pmax = 0;
+  if (!spline_desc(f, n, n_blocks, offs, lens, ncols, degrees, knots, n_der, iv, &nk, &Lmax, &pmax, &nco)) return -1;
+  if (nco * sizeof(double) > 48 * 1024) { set_err(f + ": derivative coefficients exceed 48 KB per instance"); return -1; }
+  if (B <= 0 || n_blocks == 0) return 0;
+  int n_out = 0;
+  for (int k = 0; k < n_blocks; ++k) n_out += ncols[k] * n_pts * n_der;
+  cudaStream_t stream = (cudaStream_t)stream_;
+  int device = 0;
+  CK(cudaGetDevice(&device));
+  static thread_local DescCache cache;
+  if (desc_upload(cache, device, iv, knots, nk, stream)) return -1;
+  OMG_LAUNCH(omg_eval_kernel, B, 64, sizeof(double) * nco, stream, x, B, n, n_blocks, cache.d_i, cache.d_d, n_pts,
+             tau, scale, n_der, out, n_out);
   CK(cudaGetLastError());
   return 0;
 }

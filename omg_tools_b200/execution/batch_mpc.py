@@ -28,6 +28,13 @@ is keyed by ``seed``, the MPC step and the instance, so a realisation does not d
 batch size.  history['plant'] and history['plant_input'] hold the plant state and the last
 applied input at every update boundary.  ``sample_time`` is the simulation grid of the plant
 and of the obstacle motion (the reference simulator's sample_time, 0.01 s by default).
+
+With a FreeTPoint2point (T a decision variable; Holonomic, Holonomic3D and Dubins, ideal loop) every
+instance runs the reference's free-T loop on its own motion time (point2point.py:300-374): the warm
+start re-expresses the splines with shift_spline from the instance's T [omg_shift_free_batch], only
+the instances still running are solved, the prediction samples each plan at its own
+tau = min(dt, T) / T [omg_eval_batch], and an instance stops for good when T < dt or at its goal.
+history['T'] and history['active'] hold the motion times and the instances solved at every step.
 """
 import numpy as np
 
@@ -78,6 +85,12 @@ class _HolonomicAdapter(object):
                 c = Xh[:, k * L:(k + 1) * L]
                 self.state[:, k] = c.dot(B0[0])
                 self.inp[:, k] = c.dot(B1[0])
+
+    def predict_free(self, X, idx, tau1, T, blocks):
+        """Free motion time: state and input of the instances idx (X holds their rows) at their
+        own tau1 = min(dt, T) / T, value and first derivative / T (omg_eval_batch)."""
+        out = _eval(X, blocks, tau1[:, None], T, 2).reshape(-1, self.nd, 2)   # [b][column][derivative]
+        self.state[idx], self.inp[idx] = out[:, :, 0], out[:, :, 1]
 
     def position(self):
         return self.state
@@ -175,6 +188,15 @@ def _rows(basis, tau, T, n_der):
     return np.array(rows)
 
 
+def _eval(X, blocks, tau, T, n_der):
+    """Per-instance spline values and derivatives 0..n_der-1 at the abscissae tau [B, n_pts], derivative
+    d divided by T^d (omg_eval_batch): numpy [B, columns * n_pts * n_der], column / point / derivative."""
+    import torch
+    from ..solver.b200 import eval_batch
+    t = lambda a: torch.tensor(np.ascontiguousarray(a, dtype=np.float64), device=X.device)
+    return eval_batch(X, blocks, t(tau), t(T), n_der).cpu().numpy()
+
+
 def _sample(X, L, n_col, S, device):
     """Spline columns 0..n_col-1 of every instance at the rows S [n_rows, L]: [B, n_col * n_rows]
     laid out column / row (on the device by omg_sample_batch, or on the host)."""
@@ -241,6 +263,28 @@ class _DubinsAdapter(object):
         self.state = np.c_[self.state[:, 0] + T * (vt * (1 - tg**2)).dot(wts),
                            self.state[:, 1] + T * (vt * (2 * tg)).dot(wts), 2 * np.arctan2(tg1, 1)]
         self.inp = np.c_[vt1 * q1, 2 * dtg1 / q1]
+
+    def predict_free(self, X, idx, tau1, T, blocks):
+        """Free motion time: the instances idx (X holds their rows) integrate over their own [0, tau1],
+        split at the knots below tau1; the nodes are padded with zero weights to the count of a
+        whole horizon so that one omg_eval_batch launch serves the batch (last point: tau1)."""
+        knots = np.unique(self.v.basis.knots)
+        xg, wg = np.polynomial.legendre.leggauss(self.nq)
+        nn = (len(knots) - 1) * self.nq
+        pts, wts = np.zeros((len(idx), nn + 1)), np.zeros((len(idx), nn))
+        for j, t1 in enumerate(tau1):
+            brk = [0.] + [k for k in knots if 1e-12 < k < t1 - 1e-12] + [t1]
+            nodes = np.concatenate([0.5 * (b - a) * xg + 0.5 * (a + b) for a, b in zip(brk[:-1], brk[1:])])
+            pts[j, :len(nodes)], pts[j, nn] = nodes, t1
+            wts[j, :len(nodes)] = np.concatenate([0.5 * (b - a) * wg for a, b in zip(brk[:-1], brk[1:])])
+        out = _eval(X, blocks, pts, T, 2).reshape(-1, 2, nn + 1, 2)     # [b][column][point][derivative]
+        vt, tg = out[:, 0, :nn, 0], out[:, 1, :nn, 0]
+        vt1, tg1, dtg1 = out[:, 0, nn, 0], out[:, 1, nn, 0], out[:, 1, nn, 1]
+        q1 = 1 + tg1**2
+        st = self.state[idx]
+        self.state[idx] = np.c_[st[:, 0] + T * np.einsum('bq,bq->b', vt * (1 - tg**2), wts),
+                                st[:, 1] + T * np.einsum('bq,bq->b', vt * (2 * tg), wts), 2 * np.arctan2(tg1, 1)]
+        self.inp[idx] = np.c_[vt1 * q1, 2 * dtg1 / q1]
 
     def position(self):
         return self.state[:, :2]
@@ -409,6 +453,9 @@ def plant_rows_der(basis, T, t_rel, sample_time, n_samp):
                            _rows(basis, tau, T, 4)[2:]])
 
 
+# the adapters with a per-instance prediction for a free motion time (predict_free)
+_FREE_T = ('Holonomic', 'Holonomic3D', 'Dubins')
+
 _ADAPTERS = {'Holonomic': _HolonomicAdapter, 'Holonomic3D': _HolonomicAdapter,
              'Quadrotor3D': _Quadrotor3DAdapter, 'Dubins': _DubinsAdapter,
              'HolonomicOrient': _HolonomicOrientAdapter, 'Quadrotor': _QuadrotorAdapter,
@@ -427,6 +474,16 @@ class BatchMPC(object):
     def __init__(self, problem, batch, update_time=0.1, jitter=0.0, seed=0, device_predict=True,
                  device=None, sample_time=0.01):
         import torch
+        from ..problems.point2point import FreeTPoint2point
+        self.free_T = isinstance(problem, FreeTPoint2point)
+        if self.free_T:
+            vehicle, opt = problem.vehicles[0], problem.vehicles[0].options
+            if type(vehicle).__name__ not in _FREE_T:
+                raise NotImplementedError('BatchMPC has no free end time (FreeTPoint2point) for %s'
+                                          % type(vehicle).__name__)
+            if not (opt.get('ideal_update', True) and opt.get('ideal_prediction', True)):
+                raise NotImplementedError('BatchMPC runs a free end time (FreeTPoint2point) only with '
+                                          'ideal_update and ideal_prediction on')
         self.device_predict = device_predict
         self.torch = torch
         self.problem = problem
@@ -437,8 +494,11 @@ class BatchMPC(object):
         self.update_time = update_time
         self.vehicle = problem.vehicles[0]
         self.obstacles = problem.environment.obstacles
-        self.T = problem.options['horizon_time']
-        self.knot_time = problem.knot_time
+        if self.free_T:
+            self.T = self.knot_time = None       # per instance: the variable T of every solution
+        else:
+            self.T = problem.options['horizon_time']
+            self.knot_time = problem.knot_time
         dev = device if device is not None else torch.device('cuda', self.solver.device)
         self.dev = dev
         rng = np.random.default_rng(seed)
@@ -482,6 +542,19 @@ class BatchMPC(object):
         self.closed_loop = not (self.ideal_update and self.ideal_prediction)
         if self.closed_loop:
             self._init_plant(opt, seed)
+        if self.free_T:
+            self._init_free_T()
+
+    def _init_free_T(self):
+        """Free motion time: the spline blocks of the warm start and of the prediction, the index of
+        T in x, and which instances still run (history['active'][k]: solved at step k)."""
+        from ..solver.b200 import spline_blocks
+        self.t_index = self.father._var_struct.entries[(self.problem.label, 'T')][0]
+        self.shift_blocks = spline_blocks(self.father)
+        self.veh_blocks = spline_blocks(self.father, self.vehicle)
+        self.active = np.ones(self.B, dtype=bool)
+        self.n_solved = 0
+        self.history.update({'T': [], 'active': []})
 
     def _init_plant(self, opt, seed):
         """Plant state and last applied input per instance (device tensors), the lag and the
@@ -524,6 +597,9 @@ class BatchMPC(object):
                 P[:, off[(o.label, key)]:off[(o.label, key)] + nd] = d[key]
             if 'theta' in d:
                 P[:, off[(o.label, 'theta')]] = d['theta'][:, 0]
+        if self.free_T:                 # the time axis restarts every update (point2point.py:300-306)
+            P[:, off[(self.problem.label, 't')]] = 0.
+            return
         P[:, off[(self.problem.label, 't')]] = np.round(t, 6) % self.knot_time
         P[:, off[(self.problem.label, 'T')]] = self.T
 
@@ -549,6 +625,8 @@ class BatchMPC(object):
 
     # ------------------------------------------------------------------
     def step(self):
+        if self.free_T:
+            return self._step_free_T()
         torch = self.torch
         t = self.time
         # knot crossing -> shift the warm start on the device
@@ -610,7 +688,61 @@ class BatchMPC(object):
         self.history['plant'].append(self.plant_x.cpu().numpy().copy())
         self.history['plant_input'].append(self.plant_u.cpu().numpy().copy())
 
+    def _step_free_T(self):
+        """One update of the reference's free-T loop for every active instance (Simulator.update /
+        Deployer.update with FreeTPoint2point, point2point.py:300-374): warm start by shift_spline
+        from the instance's own T (omg_shift_free_batch; not on the first step), solve the active
+        instances, predict at tau = min(dt, T) / T (omg_eval_batch), move the obstacles, and stop
+        the instances with T < dt or at their goal (check_terminal_conditions).  A stopped instance
+        is not solved again and its X, state and T stay as they are; status -1 and 0 iterations
+        stand for 'not solved' in the history."""
+        torch = self.torch
+        act = np.nonzero(self.active)[0]
+        if len(act) == 0:
+            return
+        dt = self.update_time
+        if self.n_solved > 0:
+            mask = torch.tensor(self.active.astype(np.int32), device=self.dev)
+            self.solver.shift_free_batch_device(self.X, self.shift_blocks, self.t_index, dt, active=mask)
+        self._pack_parameters(0.)
+        idx = torch.from_numpy(act).to(self.dev)
+        Xa = self.X.index_select(0, idx)
+        Pa = torch.from_numpy(self.P[act]).to(self.dev)
+        na, m = len(act), self.tb.m
+        Xn = torch.empty_like(Xa)
+        LAM = torch.empty((na, m), dtype=torch.float64, device=self.dev)
+        F = torch.empty(na, dtype=torch.float64, device=self.dev)
+        ST = torch.empty(na, dtype=torch.int32, device=self.dev)
+        IT = torch.empty(na, dtype=torch.int32, device=self.dev)
+        self.solver.solve_batch_device(Xa, Pa, self.LB, self.UB, Xn, LAM, F, ST, IT)
+        self.X.index_copy_(0, idx, Xn)
+        self.n_solved += 1
+        status, iters = np.full(self.B, -1, dtype=np.int32), np.zeros(self.B, dtype=np.int32)
+        status[act], iters[act] = ST.cpu().numpy(), IT.cpu().numpy()
+        self.history['status'].append(status)
+        self.history['iters'].append(iters)
+        self.history['active'].append(self.active.copy())
+        T = Xn[:, self.t_index].cpu().numpy()
+        self.history['T'].append(self.X[:, self.t_index].cpu().numpy().copy())
+        # the last update of an instance moves it by min(dt, T), and not at all when T is below the
+        # sample time (FreeTPoint2point.simulate, store)
+        move = T >= self.sample_time
+        if move.any():
+            sel = torch.from_numpy(np.nonzero(move)[0]).to(self.dev)
+            self.veh.predict_free(Xn.index_select(0, sel) if not move.all() else Xn, act[move],
+                                  np.minimum(dt, T[move]) / T[move], T[move], self.veh_blocks)
+        self._advance_obstacles(dt, self.sample_time)
+        self.history['state'].append(self.state.copy())
+        self.time = np.round(self.time + dt, 6)
+        tol = self.vehicle.options['stop_tol']
+        arrived = ((np.linalg.norm(self.state[act] - self.poseT[act], axis=1) <= tol) &
+                   (np.linalg.norm(self.inp[act], axis=1) <= tol))
+        self.active[act[(T < dt) | arrived]] = False
+
     def run(self, n_steps):
+        """n_steps MPC updates; with a free end time the run ends early once every instance stopped."""
         for _ in range(n_steps):
+            if self.free_T and not self.active.any():
+                break
             self.step()
         return self.history

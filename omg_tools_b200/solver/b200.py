@@ -86,7 +86,8 @@ EXPORTS = ['omg_abi_version', 'omg_last_error', 'omg_default_options',
            'omg_admm_zl_update', 'omg_sample_batch', 'omg_tables_read',
            'omg_tables_free', 'omg_integrate_rk4', 'omg_feas_batch', 'omg_feas_batch_host',
            'omg_comm_unique_id', 'omg_comm_create', 'omg_comm_destroy', 'omg_admm_exchange_x',
-           'omg_admm_zl_update_dist', 'omg_closed_loop_step', 'omg_closed_loop_step_der']
+           'omg_admm_zl_update_dist', 'omg_closed_loop_step', 'omg_closed_loop_step_der',
+           'omg_shift_free_batch', 'omg_eval_batch']
 
 _lib = None
 
@@ -146,6 +147,9 @@ def bind(lib):
     lib.omg_closed_loop_step_der.argtypes = ([C.c_int32] * 5 + [vp, C.c_int32, C.c_int32, C.c_int32, vp,
                                              C.c_double, C.c_int32, C.c_double, C.c_int32, C.c_int32,
                                              vp, vp, vp, C.c_uint64, C.c_int32] + [vp] * 8)
+    lib.omg_shift_free_batch.argtypes = [vp, C.c_int32, vp, C.c_int32, C.c_double, vp, C.c_int32] + [vp] * 6
+    lib.omg_eval_batch.argtypes = [C.c_int32, C.c_int32, vp, C.c_int32] + [vp] * 5 + [C.c_int32, vp, vp, C.c_int32,
+                                                                                    vp, vp]
     lib.omg_tables_read.argtypes = [C.c_char_p]
     lib.omg_tables_read.restype = C.POINTER(_Tables)
     lib.omg_tables_free.argtypes = [C.POINTER(_Tables)]
@@ -543,6 +547,25 @@ class B200Solver(object):
             lens.ctypes.data, ncols.ctypes.data, Tm.ctypes.data,
             _stream_handle(on_gpu, X.device, stream)))
 
+    def shift_free_batch_device(self, X, blocks, t_index, update_time, active=None, stream=None):
+        """Free-T warm start in place (omg_shift_free_batch): for every active instance of the torch
+        CUDA tensor X [B, n], shift_spline of each block by tau = u / target from its own motion
+        time X[b, t_index], which becomes target.  blocks = [(offset, len_basis, n_columns, degree,
+        knots)], e.g. spline_blocks(father); active: int32 CUDA tensor [B] (nonzero = shift) or
+        None for all."""
+        desc = _spline_desc(blocks)
+        on_gpu = _check_device_tensors((X,), self.lib)
+        if active is not None:
+            _check_int_tensors((active,))
+            if active.numel() != X.shape[0]:
+                raise ValueError('active must hold one flag per instance')
+        if X.dim() != 2 or X.shape[1] != self.n:
+            raise ValueError('X must be [B, n]')
+        self._check(self.lib.omg_shift_free_batch(
+            self._handle, X.shape[0], X.data_ptr(), int(t_index), float(update_time),
+            active.data_ptr() if active is not None else None, len(blocks),
+            *[a.ctypes.data for a in desc], _stream_handle(on_gpu, X.device, stream)))
+
     # ------------------------------------------------------------------
     # the reference's single-instance call contract
     # ------------------------------------------------------------------
@@ -656,6 +679,54 @@ def sample_batch(X, blocks, stream=None):
     rc = lib.omg_sample_batch(X.shape[0], X.shape[1], X.data_ptr(), len(blocks), offs.ctypes.data,
                               lens.ctypes.data, ncols.ctypes.data, nsamp.ctypes.data,
                               Sm.ctypes.data, out.data_ptr(), _stream_handle(on_gpu, X.device, stream))
+    if rc != 0:
+        raise RuntimeError('libomgb200: %s' % lib.omg_last_error().decode())
+    return out
+
+
+def _spline_desc(blocks):
+    """[(offset, len_basis, n_columns, degree, knots)] -> host arrays offs, lens, ncols, degrees and
+    the concatenated knots (len_basis + degree + 1 per block)."""
+    desc = [np.array([b[k] for b in blocks], dtype=np.int32) for k in range(4)]
+    knots = [np.ascontiguousarray(b[4], dtype=np.float64).reshape(-1) for b in blocks]
+    for b, k in zip(blocks, knots):
+        if k.size != b[1] + b[3] + 1:
+            raise ValueError('a block of length %d and degree %d needs %d knots, got %d'
+                             % (b[1], b[3], b[1] + b[3] + 1, k.size))
+    return desc + [np.concatenate(knots) if knots else np.zeros(1)]
+
+
+def spline_blocks(father, vehicle=None):
+    """The blocks of shift_free_batch_device / eval_batch: [(offset, len_basis, n_columns, degree,
+    knots)] of the spline variables the warm start transforms (father.shifted_entries()), or,
+    with ``vehicle``, of that vehicle's splines_seg0."""
+    out = []
+    for label, name, off, shape, _ in father.shifted_entries():
+        if vehicle is not None and (label, name) != (vehicle.label, 'splines_seg0'):
+            continue
+        basis = father.children[label]._splines_prim[name]['basis']
+        out.append((off, shape[0], shape[1], basis.degree, basis.knots))
+    return out
+
+
+def eval_batch(X, blocks, tau, scale, n_der, stream=None):
+    """Per-instance spline evaluation on the device (omg_eval_batch).  X: torch CUDA tensor
+    [B, n]; blocks = [(offset, len_basis, n_columns, degree, knots)]; tau: CUDA tensor
+    [B, n_pts] of abscissae in the knot span (padding points anywhere; they evaluate to 0 outside
+    it); scale: CUDA tensor [B].  Returns a CUDA tensor [B, sum(n_columns) * n_pts * n_der] laid
+    out block / column / point / derivative, derivative d divided by scale^d."""
+    import torch
+    lib = load_library()
+    desc = _spline_desc(blocks)
+    on_gpu = _check_device_tensors((X, tau, scale), lib)
+    B = X.shape[0]
+    if X.dim() != 2 or tau.dim() != 2 or tau.shape[0] != B or scale.numel() != B:
+        raise ValueError('X must be [B, n], tau [B, n_pts] and scale [B]')
+    n_pts = tau.shape[1]
+    out = torch.empty((B, int(desc[2].sum()) * n_pts * int(n_der)), dtype=torch.float64, device=X.device)
+    rc = lib.omg_eval_batch(B, X.shape[1], X.data_ptr(), len(blocks), *[a.ctypes.data for a in desc], n_pts,
+                            tau.data_ptr(), scale.data_ptr(), int(n_der), out.data_ptr(),
+                            _stream_handle(on_gpu, X.device, stream))
     if rc != 0:
         raise RuntimeError('libomgb200: %s' % lib.omg_last_error().decode())
     return out
