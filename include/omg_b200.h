@@ -360,6 +360,38 @@ int omg_closed_loop_step_der(int32_t model, int32_t B, int32_t n_state, int32_t 
                              const double* plant_u, double* plant_x_next, double* plant_u_next,
                              double* pred_x, double* pred_u, double* scratch, void* stream);
 
+/* omg_closed_loop_step_der with a free motion time (reference FreeTPoint2point.store / simulate,
+ * point2point.py:313-346, on Vehicle.store / predict / simulate): every instance samples its own
+ * plan on its own time axis, so no basis row is shared and the rows are built on the device.
+ * DEVICE: x [B x n], plant_x, plant_u, the four outputs and scratch as omg_closed_loop_step_der;
+ * scratch holds B x n_input x (max n_traj + 24) doubles (disturb only).  The input splines are
+ * the first n_input columns of ONE spline block described as omg_eval_batch describes it:
+ * spl_offset in x, basis length L, n_cols columns, degree, HOST knots [L + degree + 1].
+ * Instance b reads its motion time T_b = x[b, t_index] on the device and takes its planned input
+ * at samples s = 0..n_samp[b] from the values and derivatives of the columns at s*sample_time /
+ * T_b, derivative d divided by T_b^d (the rows of the reference's store on
+ * linspace(0, (n_traj-1)*sample_time, n_traj)), through the model's input map
+ * (omg_closed_loop_step_der; n_der from the model's to 4, at most degree + 1).
+ * HOST int32 n_samp [B]: samples of the update of b, min(update_time, T_b) / sample_time; 0 =
+ * nothing is written for b (a stopped instance, or T_b below the sample time).  HOST int32
+ * n_traj [B] (read with disturb only): length of b's stored trajectory, T_b / sample_time + 1,
+ * over which its disturbance is filtered; 0 = no disturbance for b.  The noise is keyed by
+ * (seed, step, b, signal, pair) with b the row of x: a realisation belongs to the instance and
+ * does not depend on which other rows are stepped.  Filter, lag and RK4 are
+ * omg_closed_loop_step_der's.  Rejected with a message: everything omg_closed_loop_step_der
+ * rejects, a spline block outside x or with fewer than n_input columns, t_index outside x,
+ * n_samp[b] < 0, 0 < n_traj[b] <= 12 (filtfilt's padding), 0 < n_traj[b] < n_samp[b] + 1, and
+ * (max n_samp + 1) * n_input > 2048. */
+int omg_closed_loop_step_free(int32_t model, int32_t B, int32_t n_state, int32_t n_input, int32_t n,
+                              const double* x, int32_t spl_offset, int32_t L, int32_t n_cols,
+                              int32_t degree, const double* knots, int32_t t_index, int32_t n_der,
+                              const int32_t* n_samp, const int32_t* n_traj, double sample_time,
+                              int32_t lag, double time_constant, int32_t disturb, const double* filt,
+                              const double* mean, const double* stdev, uint64_t seed, int32_t step,
+                              const double* plant_x, const double* plant_u, double* plant_x_next,
+                              double* plant_u_next, double* pred_x, double* pred_u, double* scratch,
+                              void* stream);
+
 /* ADMM consensus step for n_agents agents on the current device (DEVICE pointers):
  * closed-form z-update, lambda-update and squared residuals of the reference's
  * ADMM updater (omgtools/problems/admm.py:117-168 construct_upd_z/update_z,

@@ -1352,8 +1352,40 @@ __device__ __forceinline__ double omg_row_dot(const double* r, const double* c, 
   return acc;
 }
 
-// One block per instance.  Both halves start from the plant state x_p(t_k) and the trajectory
-// just solved, sampled at t_k + s*dt, s = 0..n_samp:
+// Planned input of one sample (each vehicle's splines2signals): v[d][c] is the d-th derivative of
+// the input spline column c at the sample, divided by T^d.
+__device__ __forceinline__ void omg_cl_input_map(int model, int ni, const double (*v)[OMG_CL_MAX_INPUT], double* u) {
+  if (model == OMG_ODE_QUADROTOR2D) {               // quadrotor.py splines2signals
+    const double ddx = v[2][0], ddy = v[2][1], dddx = v[3][0], dddy = v[3][1];
+    const double ay = ddy + 9.81;
+    u[0] = sqrt(ddx * ddx + ay * ay);
+    u[1] = (dddx * ay - ddx * dddy) / (ay * ay + ddx * ddx);
+  } else if (model == OMG_ODE_DUBINS) {             // dubins.py: v = v~ (1 + tg^2), w = 2 tg' / (1 + tg^2)
+    const double vt = v[0][0], tg = v[0][1], dtg = v[1][1], q = 1.0 + tg * tg;
+    u[0] = vt * q; u[1] = 2.0 * dtg / q;
+  } else if (model == OMG_ODE_HOLONOMIC_ORIENT) {   // holonomicorient.py: (x', y', 2 tg' / (1 + tg^2))
+    const double tg = v[0][2];
+    u[0] = v[1][0]; u[1] = v[1][1];
+    u[2] = 2.0 * v[1][2] / (1.0 + tg * tg);
+  } else if (model == OMG_ODE_SIMPLE_QUADROTOR3D) { // quadrotor3d_simple.py splines2signals
+    const double ddx = v[2][0], ddy = v[2][1], dddx = v[3][0], dddy = v[3][1];
+    const double az = v[2][2] + 9.81, dddz = v[3][2];
+    const double h2 = ddx * ddx + az * az, f2 = ddx * ddx + ddy * ddy + az * az;
+    u[0] = sqrt(f2);
+    u[1] = (-dddy * h2 + ddy * (ddx * dddx + dddz * az)) / (f2 * sqrt(h2));
+    u[2] = (az * dddx - ddx * dddz) / (az * az + ddx * ddx);
+  } else if (model == OMG_ODE_QUADROTOR3D) {
+    const double f = v[0][0], qp = v[0][1], qt = v[0][2], dqp = v[1][1], dqt = v[1][2];
+    const double ep = 1.0 + qp * qp, et = 1.0 + qt * qt;
+    u[0] = f * (ep * et); u[1] = 2.0 * dqp / ep; u[2] = 2.0 * dqt / et;
+  } else {
+    for (int c = 0; c < ni; ++c) u[c] = v[1][c];
+  }
+}
+
+// The part of one instance's plant step that follows the planned inputs U [n_samp+1][ni] (shared
+// memory, complete at entry or completed by the caller's threads before the barrier below), run
+// by every thread of the block:
 //   simulate: planned input + filtered noise -> first-order lag -> RK4 of the ODE -> x_p(t_k+1)
 //   predict:  planned input -> RK4 of the ODE from x_p(t_k) -> state0 of the next solve
 // RK4 takes the linearly interpolated input of the reference's interp1d: u_i, the mean of
@@ -1361,72 +1393,19 @@ __device__ __forceinline__ double omg_row_dot(const double* r, const double* c, 
 // filtered over the whole stored trajectory (n_traj samples) by the reference's
 // filtfilt(butter(3, fc)): odd extension by 12, forward and backward passes of the transposed
 // direct form from zi * (first value); only samples 0..n_samp are kept.
-// filt = {b0..b3, a0..a3 (a0 = 1), zi0..zi2}; scratch holds one forward pass per series.
-// R = [n_der][n_samp+1][L]: row d is the d-th derivative of the basis divided by T^d.  `model`
-// selects the planned-input map, `ode` the right-hand side (omg_ode_models).
-__global__ void omg_closed_loop_kernel(int model, int ode, int ns, int ni, int n, const double* __restrict__ x,
-                                       int L, int n_samp, const double* __restrict__ R,
-                                       double dt, int lag, double tau, int disturb, int n_traj,
-                                       const double* __restrict__ filt, const double* __restrict__ mean,
-                                       const double* __restrict__ stdev, uint64_t seed, int step,
-                                       const double* plant_x, const double* plant_u,    // (may alias the next)
-                                       double* plant_x_next, double* plant_u_next,
-                                       double* __restrict__ pred_x, double* __restrict__ pred_u,
-                                       double* __restrict__ scratch) {
-  OMG_DYN_SHARED(sm);
-  const int b = blockIdx.x, ts = n_samp + 1;
-  double* U = sm;                // planned input [ts][ni]
-  double* D = sm + ts * ni;      // filtered disturbance [ts][ni]
-  double* A = sm + 2 * ts * ni;  // input reaching the ODE [ts][ni]
-  const double* xb = x + (size_t)b * n;
-  // planned inputs (splines2signals of each vehicle); row d carries the 1/T^d
-  const size_t nr = (size_t)ts * L;
-  for (int s = threadIdx.x; s < ts; s += blockDim.x) {
-    const double* r0 = R + (size_t)s * L;
-    const double* r1 = r0 + nr;
-    if (model == OMG_ODE_QUADROTOR2D) {             // quadrotor.py splines2signals
-      const double *r2 = r0 + 2 * nr, *r3 = r0 + 3 * nr;
-      const double ddx = omg_row_dot(r2, xb, L), ddy = omg_row_dot(r2, xb + L, L);
-      const double dddx = omg_row_dot(r3, xb, L), dddy = omg_row_dot(r3, xb + L, L);
-      const double ay = ddy + 9.81;
-      U[s * 2] = sqrt(ddx * ddx + ay * ay);
-      U[s * 2 + 1] = (dddx * ay - ddx * dddy) / (ay * ay + ddx * ddx);
-    } else if (model == OMG_ODE_DUBINS) {           // dubins.py: v = v~ (1 + tg^2), w = 2 tg' / (1 + tg^2)
-      const double vt = omg_row_dot(r0, xb, L), tg = omg_row_dot(r0, xb + L, L);
-      const double dtg = omg_row_dot(r1, xb + L, L), q = 1.0 + tg * tg;
-      U[s * 2] = vt * q; U[s * 2 + 1] = 2.0 * dtg / q;
-    } else if (model == OMG_ODE_HOLONOMIC_ORIENT) { // holonomicorient.py: (x', y', 2 tg' / (1 + tg^2))
-      const double tg = omg_row_dot(r0, xb + 2 * L, L);
-      U[s * 3] = omg_row_dot(r1, xb, L); U[s * 3 + 1] = omg_row_dot(r1, xb + L, L);
-      U[s * 3 + 2] = 2.0 * omg_row_dot(r1, xb + 2 * L, L) / (1.0 + tg * tg);
-    } else if (model == OMG_ODE_SIMPLE_QUADROTOR3D) {   // quadrotor3d_simple.py splines2signals
-      const double *r2 = r0 + 2 * nr, *r3 = r0 + 3 * nr;
-      const double ddx = omg_row_dot(r2, xb, L), ddy = omg_row_dot(r2, xb + L, L);
-      const double dddx = omg_row_dot(r3, xb, L), dddy = omg_row_dot(r3, xb + L, L);
-      const double az = omg_row_dot(r2, xb + 2 * L, L) + 9.81, dddz = omg_row_dot(r3, xb + 2 * L, L);
-      const double h2 = ddx * ddx + az * az, f2 = ddx * ddx + ddy * ddy + az * az;
-      U[s * 3] = sqrt(f2);
-      U[s * 3 + 1] = (-dddy * h2 + ddy * (ddx * dddx + dddz * az)) / (f2 * sqrt(h2));
-      U[s * 3 + 2] = (az * dddx - ddx * dddz) / (az * az + ddx * ddx);
-    } else if (model == OMG_ODE_QUADROTOR3D) {
-      double f = 0.0, qp = 0.0, qt = 0.0, dqp = 0.0, dqt = 0.0;
-      for (int k = 0; k < L; ++k) {
-        f += r0[k] * xb[k]; qp += r0[k] * xb[L + k]; qt += r0[k] * xb[2 * L + k];
-        dqp += r1[k] * xb[L + k]; dqt += r1[k] * xb[2 * L + k];
-      }
-      const double ep = 1.0 + qp * qp, et = 1.0 + qt * qt;
-      U[s * 3] = f * (ep * et); U[s * 3 + 1] = 2.0 * dqp / ep; U[s * 3 + 2] = 2.0 * dqt / et;
-    } else {
-      for (int c = 0; c < ni; ++c) {
-        double acc = 0.0;
-        for (int k = 0; k < L; ++k) acc += r1[k] * xb[c * L + k];
-        U[s * ni + c] = acc;
-      }
-    }
-  }
+// filt = {b0..b3, a0..a3 (a0 = 1), zi0..zi2}; scratch holds one forward pass per series, `stride`
+// doubles apart (at least n_traj + 24).  D, A: [n_samp+1][ni] of shared memory.  The noise is
+// keyed by (seed, step, b, signal, pair).
+__device__ void omg_cl_tail(int b, int ode, int ns, int ni, int n_samp, double dt, int lag, double tau,
+                            int disturb, int n_traj, const double* __restrict__ filt,
+                            const double* __restrict__ mean, const double* __restrict__ stdev, uint64_t seed,
+                            int step, const double* plant_x, const double* plant_u, double* plant_x_next,
+                            double* plant_u_next, double* __restrict__ pred_x, double* __restrict__ pred_u,
+                            double* __restrict__ scratch, size_t stride, const double* U, double* D, double* A) {
+  const int ts = n_samp + 1;
   if (disturb && (int)threadIdx.x < ni) {
     const int j = threadIdx.x, N = n_traj + 2 * OMG_CL_PAD;
-    double* e = scratch + ((size_t)b * ni + j) * N;
+    double* e = scratch + ((size_t)b * ni + j) * stride;
     double* w = e + OMG_CL_PAD;                     // white noise at 0..n_traj-1
     for (int p = 0; 2 * p < n_traj; ++p) {
       double z0, z1;
@@ -1498,6 +1477,36 @@ __global__ void omg_closed_loop_kernel(int model, int ode, int ns, int ni, int n
   double* uo = simulate ? plant_u_next : pred_u;
   for (int j = 0; j < ns; ++j) xo[(size_t)b * ns + j] = y[j];
   for (int c = 0; c < ni; ++c) uo[(size_t)b * ni + c] = Uin[n_samp * ni + c];
+}
+
+// One block per instance; both halves start from the plant state x_p(t_k) and the trajectory
+// just solved, sampled at t_k + s*dt, s = 0..n_samp (omg_cl_tail).  R = [nd][n_samp+1][L]: row d
+// is the d-th derivative of the basis divided by T^d, nd the rows the model reads.  `model`
+// selects the planned-input map, `ode` the right-hand side (omg_ode_models).
+__global__ void omg_closed_loop_kernel(int model, int ode, int nd, int ns, int ni, int n, const double* __restrict__ x,
+                                       int L, int n_samp, const double* __restrict__ R,
+                                       double dt, int lag, double tau, int disturb, int n_traj,
+                                       const double* __restrict__ filt, const double* __restrict__ mean,
+                                       const double* __restrict__ stdev, uint64_t seed, int step,
+                                       const double* plant_x, const double* plant_u,    // (may alias the next)
+                                       double* plant_x_next, double* plant_u_next,
+                                       double* __restrict__ pred_x, double* __restrict__ pred_u,
+                                       double* __restrict__ scratch) {
+  OMG_DYN_SHARED(sm);
+  const int b = blockIdx.x, ts = n_samp + 1;
+  double* U = sm;                // planned input [ts][ni]
+  double* D = sm + ts * ni;      // filtered disturbance [ts][ni]
+  double* A = sm + 2 * ts * ni;  // input reaching the ODE [ts][ni]
+  const double* xb = x + (size_t)b * n;
+  const size_t nr = (size_t)ts * L;
+  for (int s = threadIdx.x; s < ts; s += blockDim.x) {
+    double v[4][OMG_CL_MAX_INPUT];
+    for (int d = 0; d < nd; ++d)
+      for (int c = 0; c < ni; ++c) v[d][c] = omg_row_dot(R + d * nr + (size_t)s * L, xb + c * L, L);
+    omg_cl_input_map(model, ni, v, U + s * ni);
+  }
+  omg_cl_tail(b, ode, ns, ni, n_samp, dt, lag, tau, disturb, n_traj, filt, mean, stdev, seed, step, plant_x,
+              plant_u, plant_x_next, plant_u_next, pred_x, pred_u, scratch, (size_t)n_traj + 2 * OMG_CL_PAD, U, D, A);
 }
 
 // trajectory sampling: out[b, blk, c, s] = sum_k S_blk[s,k] * x[b, off_blk + c*len_blk + k]
@@ -1732,6 +1741,64 @@ __global__ void omg_eval_kernel(const double* __restrict__ x, int B, int n, int 
     }
     ooff += nc * n_pts * n_der;
   }
+}
+
+// Closed-loop plant step with a free motion time, one instance per block: omg_closed_loop_kernel
+// with the planned inputs of instance b sampled on its own time axis, s*dt / T_b for
+// s = 0..n_samp[b], T_b = x[b, t_index], by the derivative coefficients and Cox-de Boor values of
+// omg_eval_kernel (derivative d divided by T_b^d).  desc = {offset in x, L, columns, degree} of the
+// spline block whose first ni columns are the input splines, kn its L + p + 1 knots.  n_samp[b] = 0:
+// nothing is written for b; n_traj[b] = 0: no disturbance for b.  Shared memory: U, D, A
+// [ts_max][ni] | derivative coefficients [ni][nd][L].
+__global__ void omg_closed_loop_free_kernel(int model, int ode, int nd, int ns, int ni, int n,
+                                            const double* __restrict__ x, const int* __restrict__ desc,
+                                            const double* __restrict__ kn, int t_index,
+                                            const int* __restrict__ n_samp, const int* __restrict__ n_traj,
+                                            int ts_max, double dt, int lag, double tau, int disturb,
+                                            const double* __restrict__ filt, const double* __restrict__ mean,
+                                            const double* __restrict__ stdev, uint64_t seed, int step,
+                                            const double* plant_x, const double* plant_u,
+                                            double* plant_x_next, double* plant_u_next,
+                                            double* __restrict__ pred_x, double* __restrict__ pred_u,
+                                            double* __restrict__ scratch, size_t stride) {
+  OMG_DYN_SHARED(sm);
+  const int b = blockIdx.x, t = threadIdx.x, nt = blockDim.x, nsb = n_samp[b];
+  if (nsb <= 0) return;
+  const int ts = nsb + 1, off = desc[0], L = desc[1], p = desc[3];
+  double* U = sm;
+  double* D = sm + (size_t)ts_max * ni;
+  double* A = sm + 2 * (size_t)ts_max * ni;
+  double* cd = sm + 3 * (size_t)ts_max * ni;
+  const double* xb = x + (size_t)b * n;
+  const double T = xb[t_index];
+  for (int c = t; c < ni; c += nt) {                // de Boor X.16, as omg_eval_kernel
+    double* q = cd + (size_t)c * nd * L;
+    for (int i = 0; i < L; ++i) q[i] = xb[off + c * L + i];
+    for (int d = 1; d < nd; ++d)
+      for (int j = 0; j < L - d; ++j) {
+        const double den = kn[j + p + 1] - kn[j + d];
+        q[d * L + j] = den != 0.0 ? (p - d + 1) * (q[(d - 1) * L + j + 1] - q[(d - 1) * L + j]) / den : 0.0;
+      }
+  }
+  __syncthreads();
+  for (int s = t; s < ts; s += nt) {
+    const double xs = (double)s * dt / T;
+    double w[OMG_SPL_MAX_LEN + OMG_SPL_MAX_DEGREE], v[4][OMG_CL_MAX_INPUT], sd = 1.0;
+    for (int d = 0; d < nd; ++d) {
+      omg_cox_de_boor(kn + d, p - d, xs, 0, L - d, w);
+      for (int c = 0; c < ni; ++c) {
+        const double* q = cd + ((size_t)c * nd + d) * L;
+        double acc = 0.0;
+        for (int i = 0; i < L - d; ++i) acc += w[i] * q[i];
+        v[d][c] = acc / sd;
+      }
+      sd *= T;
+    }
+    omg_cl_input_map(model, ni, v, U + s * ni);
+  }
+  const int ntr = n_traj ? n_traj[b] : 0;
+  omg_cl_tail(b, ode, ns, ni, nsb, dt, lag, tau, disturb && ntr > 0, ntr, filt, mean, stdev, seed, step, plant_x,
+              plant_u, plant_x_next, plant_u_next, pred_x, pred_u, scratch, stride, U, D, A);
 }
 
 // ---------------------------------------------------------------------------
@@ -2863,7 +2930,8 @@ static int closed_loop_launch(const char* fn, int32_t model, int32_t B, int32_t 
   if (desc_upload(cache, device, std::vector<int>(1, 0), dv.data(), dv.size(), stream)) return -1;
   const double* d = cache.d_d;
   const size_t smem = sizeof(double) * 3 * (size_t)(n_samp + 1) * n_input;
-  OMG_LAUNCH(omg_closed_loop_kernel, B, 32, smem, stream, model, omg_ode_models[model].ode, n_state, n_input, n, x,
+  OMG_LAUNCH(omg_closed_loop_kernel, B, 32, smem, stream, model, omg_ode_models[model].ode,
+             omg_ode_models[model].n_der, n_state, n_input, n, x,
              L, n_samp, d, sample_time, lag, time_constant, disturb, n_traj, d + nR, d + nR + 11,
              d + nR + 11 + n_input, seed, step, plant_x, plant_u, plant_x_next, plant_u_next, pred_x, pred_u, scratch);
   CK(cudaGetLastError());
@@ -2893,6 +2961,81 @@ int omg_closed_loop_step(int32_t model, int32_t B, int32_t n_state, int32_t n_in
   return closed_loop_launch("omg_closed_loop_step", model, B, n_state, n_input, n, x, L, n_samp, 2, R0, R1,
                             sample_time, lag, time_constant, disturb, n_traj, filt, mean, stdev, seed, step, plant_x,
                             plant_u, plant_x_next, plant_u_next, pred_x, pred_u, scratch, stream);
+}
+
+int omg_closed_loop_step_free(int32_t model, int32_t B, int32_t n_state, int32_t n_input, int32_t n, const double* x,
+                              int32_t spl_offset, int32_t L, int32_t n_cols, int32_t degree, const double* knots,
+                              int32_t t_index, int32_t n_der, const int32_t* n_samp, const int32_t* n_traj,
+                              double sample_time, int32_t lag, double time_constant, int32_t disturb,
+                              const double* filt, const double* mean, const double* stdev, uint64_t seed, int32_t step,
+                              const double* plant_x, const double* plant_u, double* plant_x_next, double* plant_u_next,
+                              double* pred_x, double* pred_u, double* scratch, void* stream_) {
+  const std::string f("omg_closed_loop_step_free");
+  if (model < 0 || model >= OMG_ODE_N_MODELS) { set_err(f + ": unknown vehicle model " + std::to_string(model)); return -1; }
+  const bool sizes_ok = omg_ode_sizes_ok(model, n_state, n_input) && n_input <= OMG_CL_MAX_INPUT;
+  if (!sizes_ok || B < 0) { set_err(f + ": bad state / input sizes"); return -1; }
+  if (n_der < omg_ode_models[model].n_der || n_der > 4) {
+    set_err(f + ": vehicle model " + std::to_string(model) + " needs " + std::to_string(omg_ode_models[model].n_der) +
+            " to 4 derivative rows, got " + std::to_string(n_der)); return -1; }
+  if (!x || !knots || !n_samp || !plant_x || !plant_u || !plant_x_next || !plant_u_next || !pred_x || !pred_u ||
+      (disturb && (!n_traj || !filt || !mean || !stdev || !scratch))) { set_err(f + ": null argument"); return -1; }
+  std::vector<int> iv;
+  size_t nk = 0, nco = 0;
+  int Lmax = 1, pmax = 0;
+  if (!spline_desc(f, n, 1, &spl_offset, &L, &n_cols, &degree, knots, n_der, iv, &nk, &Lmax, &pmax, &nco)) return -1;
+  if (n_cols < n_input) {
+    set_err(f + ": the spline block has " + std::to_string(n_cols) + " columns, the model reads " +
+            std::to_string(n_input)); return -1; }
+  if (t_index < 0 || t_index >= n) {
+    set_err(f + ": t_index " + std::to_string(t_index) + " outside [0, " + std::to_string(n) + ")"); return -1; }
+  if (!(sample_time > 0.0)) { set_err(f + ": sample_time must be > 0"); return -1; }
+  if (lag && !(time_constant > 0.0)) { set_err(f + ": time_constant must be > 0 with the lag on"); return -1; }
+  int ns_max = 0, nt_max = 0;
+  for (int b = 0; b < B; ++b) {
+    const std::string inst = f + ": instance " + std::to_string(b) + ": ";
+    if (n_samp[b] < 0) { set_err(inst + "n_samp < 0"); return -1; }
+    ns_max = std::max(ns_max, (int)n_samp[b]);
+    if (!disturb) continue;
+    const int nt = n_traj[b];
+    if (nt < 0 || (nt > 0 && nt <= OMG_CL_PAD)) {
+      set_err(inst + "n_traj must be 0 or exceed the filter padding of 12 samples"); return -1; }
+    if (nt > 0 && nt < n_samp[b] + 1) { set_err(inst + "n_traj < n_samp + 1"); return -1; }
+    nt_max = std::max(nt_max, nt);
+  }
+  // three [n_samp+1][n_input] arrays for the largest update
+  if ((int64_t)(ns_max + 1) * n_input > 2048) {
+    set_err(f + ": (max n_samp + 1) * n_input exceeds 2048 samples per update"); return -1; }
+  if (B == 0 || ns_max == 0) return 0;
+  cudaStream_t stream = (cudaStream_t)stream_;
+  // host descriptors -> device: ints {desc (4) | n_samp [B] | n_traj [B]}, doubles {knots | filt (11) | mean | stdev}
+  std::vector<int> di(4 + 2 * (size_t)B, 0);
+  std::copy(iv.begin(), iv.begin() + 4, di.begin());
+  std::copy(n_samp, n_samp + B, di.begin() + 4);
+  if (disturb) std::copy(n_traj, n_traj + B, di.begin() + 4 + B);
+  std::vector<double> dv(nk + 11 + 2 * (size_t)n_input, 0.0);
+  std::copy(knots, knots + nk, dv.begin());
+  if (disturb) {
+    std::copy(filt, filt + 11, dv.begin() + nk);
+    std::copy(mean, mean + n_input, dv.begin() + nk + 11);
+    std::copy(stdev, stdev + n_input, dv.begin() + nk + 11 + n_input);
+  }
+  int device = 0;
+  CK(cudaGetDevice(&device));
+  static thread_local DescCache cache;
+  if (desc_upload(cache, device, di, dv.data(), dv.size(), stream)) return -1;
+  const int* d_i = cache.d_i;
+  const double* d = cache.d_d;
+  const int ts_max = ns_max + 1;
+  const size_t smem = sizeof(double) * (3 * (size_t)ts_max * n_input + (size_t)n_input * n_der * L);
+  if (smem > 48 * 1024)
+    CK(cudaFuncSetAttribute((const void*)omg_closed_loop_free_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                            (int)smem));
+  OMG_LAUNCH(omg_closed_loop_free_kernel, B, 32, smem, stream, model, omg_ode_models[model].ode, n_der, n_state,
+             n_input, n, x, d_i, d, t_index, d_i + 4, d_i + 4 + B, ts_max, sample_time, lag, time_constant, disturb,
+             d + nk, d + nk + 11, d + nk + 11 + n_input, seed, step, plant_x, plant_u, plant_x_next, plant_u_next,
+             pred_x, pred_u, scratch, (size_t)nt_max + 2 * OMG_CL_PAD);
+  CK(cudaGetLastError());
+  return 0;
 }
 
 int omg_admm_zl_update(int32_t n_agents, int32_t nsh, int32_t n_nghb, int32_t L,

@@ -29,12 +29,20 @@ batch size.  history['plant'] and history['plant_input'] hold the plant state an
 applied input at every update boundary.  ``sample_time`` is the simulation grid of the plant
 and of the obstacle motion (the reference simulator's sample_time, 0.01 s by default).
 
-With a FreeTPoint2point (T a decision variable; Holonomic, Holonomic3D and Dubins, ideal loop) every
-instance runs the reference's free-T loop on its own motion time (point2point.py:300-374): the warm
-start re-expresses the splines with shift_spline from the instance's T [omg_shift_free_batch], only
-the instances still running are solved, the prediction samples each plan at its own
+With a FreeTPoint2point (T a decision variable; Holonomic, Holonomic3D and Dubins) every instance
+runs the reference's free-T loop on its own motion time (point2point.py:300-374): the warm start
+re-expresses the splines with shift_spline from the instance's T [omg_shift_free_batch], only the
+instances still running are solved, the prediction samples each plan at its own
 tau = min(dt, T) / T [omg_eval_batch], and an instance stops for good when T < dt or at its goal.
 history['T'] and history['active'] hold the motion times and the instances solved at every step.
+The free-T loop runs ideal, or closed with ideal_prediction off (ideal_update on or off): one launch
+[omg_closed_loop_step_free] on the whole batch samples each moving instance's plan on its own time
+axis for min(dt, T) / sample_time samples and filters its disturbance over its own stored trajectory,
+T / sample_time + 1 samples; state0 of the next solve is the kernel's prediction, and the stop test
+reads the plant, as the reference's check_terminal_conditions reads signals.  A final update with at
+most 12 trajectory samples (T < 0.12 s at 0.01 s samples), where the reference's filtfilt would raise,
+gets no disturbance.  ideal_update off with ideal_prediction on raises: that prediction never looks at
+the plant, while the free-T stop test reads it.
 """
 import numpy as np
 
@@ -481,9 +489,10 @@ class BatchMPC(object):
             if type(vehicle).__name__ not in _FREE_T:
                 raise NotImplementedError('BatchMPC has no free end time (FreeTPoint2point) for %s'
                                           % type(vehicle).__name__)
-            if not (opt.get('ideal_update', True) and opt.get('ideal_prediction', True)):
+            if not opt.get('ideal_update', True) and opt.get('ideal_prediction', True):
+                # the ideal prediction never looks at the plant, while the stop test reads it
                 raise NotImplementedError('BatchMPC runs a free end time (FreeTPoint2point) only with '
-                                          'ideal_update and ideal_prediction on')
+                                          'ideal_update and ideal_prediction on, or with ideal_prediction off')
         self.device_predict = device_predict
         self.torch = torch
         self.problem = problem
@@ -576,7 +585,8 @@ class BatchMPC(object):
             ni = self.plant_u.shape[1]
             stdev = np.broadcast_to(np.asarray(dist['stdev'], dtype=float), (ni,))
             mean = np.broadcast_to(np.asarray(dist.get('mean', np.zeros(ni)), dtype=float), (ni,))
-            n_traj = int(np.round(self.T / sample_time, 6)) + 1
+            # (a free motion time grows the scratch with the longest trajectory of a step)
+            n_traj = int(np.round(self.T / sample_time, 6)) + 1 if self.T is not None else 0
             scratch = torch.empty(self.B * ni * (n_traj + 24), dtype=torch.float64, device=self.dev)
             self.disturbance = (disturbance_filter(dist['fc']), mean, stdev, scratch)
         self.history['plant'] = [self.plant_x.cpu().numpy().copy()]
@@ -727,17 +737,63 @@ class BatchMPC(object):
         # the last update of an instance moves it by min(dt, T), and not at all when T is below the
         # sample time (FreeTPoint2point.simulate, store)
         move = T >= self.sample_time
-        if move.any():
+        if self.closed_loop:
+            self._plant_step_free(act, move, T)
+        if move.any() and (not self.closed_loop or self.ideal_update):
             sel = torch.from_numpy(np.nonzero(move)[0]).to(self.dev)
             self.veh.predict_free(Xn.index_select(0, sel) if not move.all() else Xn, act[move],
                                   np.minimum(dt, T[move]) / T[move], T[move], self.veh_blocks)
+        if self.closed_loop:
+            moved = act[move]
+            if self.ideal_update and len(moved):
+                sel = torch.from_numpy(moved).to(self.dev)
+                self.plant_x.index_copy_(0, sel, torch.from_numpy(self.state[moved]).to(self.dev))
+                self.plant_u.index_copy_(0, sel, torch.from_numpy(self.inp[moved]).to(self.dev))
+            # (ideal_prediction is off: state0 of the next solve is the kernel's prediction)
+            self.veh.state[moved] = self.pred_x.cpu().numpy()[moved]
+            self.veh.inp[moved] = self.pred_u.cpu().numpy()[moved]
+            px, pu = self.plant_x.cpu().numpy().copy(), self.plant_u.cpu().numpy().copy()
+            self.history['plant'].append(px)
+            self.history['plant_input'].append(pu)
+            # the reference's check_terminal_conditions reads the plant (signals)
+            pos, inp = px[act], pu[act]
+        else:
+            pos, inp = self.state[act], self.inp[act]
         self._advance_obstacles(dt, self.sample_time)
         self.history['state'].append(self.state.copy())
         self.time = np.round(self.time + dt, 6)
         tol = self.vehicle.options['stop_tol']
-        arrived = ((np.linalg.norm(self.state[act] - self.poseT[act], axis=1) <= tol) &
-                   (np.linalg.norm(self.inp[act], axis=1) <= tol))
+        arrived = ((np.linalg.norm(pos - self.poseT[act], axis=1) <= tol) &
+                   (np.linalg.norm(inp, axis=1) <= tol))
         self.active[act[(T < dt) | arrived]] = False
+
+    def _plant_step_free(self, act, move, T):
+        """Reference Vehicle.simulate and predict of every instance that moves in this update
+        (FreeTPoint2point.store / simulate) in one launch on the whole batch [omg_closed_loop_step_free]:
+        instance b samples its plan on its own time axis for min(dt, T_b) / sample_time samples and
+        filters its disturbance over its own stored trajectory, T_b / sample_time + 1 samples.  An
+        instance that is stopped or whose T is below the sample time is not touched.  The one
+        deviation from the reference: a final update with T_b / sample_time + 1 <= 12 samples (T below
+        0.12 s at 0.01 s samples), where the reference's filtfilt would raise, gets no disturbance."""
+        from ..solver.b200 import closed_loop_step_free
+        st, dt = self.sample_time, self.update_time
+        n_samp, n_traj = np.zeros(self.B, dtype=np.int32), np.zeros(self.B, dtype=np.int32)
+        Tm, am = T[move], act[move]
+        n_samp[am] = np.round(np.minimum(dt, Tm) / st, 6).astype(np.int32)
+        n_traj[am] = np.round(Tm / st, 6).astype(np.int32) + 1
+        n_traj[n_traj <= 12] = 0
+        dist = None
+        if self.disturbance is not None:
+            filt, mean, stdev, scratch = self.disturbance
+            need = self.B * self.plant_u.shape[1] * (int(n_traj.max()) + 24)
+            if scratch.numel() < need:
+                scratch = self.torch.empty(need, dtype=self.torch.float64, device=self.dev)
+                self.disturbance = (filt, mean, stdev, scratch)
+            dist = (filt, mean, stdev, n_traj, scratch)
+        closed_loop_step_free(self.model, self.X, self.veh_blocks[0], self.t_index, self.veh.N_DER, n_samp, st,
+                              self.plant_x, self.plant_u, (self.plant_x, self.plant_u, self.pred_x, self.pred_u),
+                              self.k, seed=self.seed, time_constant=self.time_constant, disturbance=dist)
+        self.k += 1
 
     def run(self, n_steps):
         """n_steps MPC updates; with a free end time the run ends early once every instance stopped."""

@@ -87,7 +87,7 @@ EXPORTS = ['omg_abi_version', 'omg_last_error', 'omg_default_options',
            'omg_tables_free', 'omg_integrate_rk4', 'omg_feas_batch', 'omg_feas_batch_host',
            'omg_comm_unique_id', 'omg_comm_create', 'omg_comm_destroy', 'omg_admm_exchange_x',
            'omg_admm_zl_update_dist', 'omg_closed_loop_step', 'omg_closed_loop_step_der',
-           'omg_shift_free_batch', 'omg_eval_batch']
+           'omg_shift_free_batch', 'omg_eval_batch', 'omg_closed_loop_step_free']
 
 _lib = None
 
@@ -147,6 +147,9 @@ def bind(lib):
     lib.omg_closed_loop_step_der.argtypes = ([C.c_int32] * 5 + [vp, C.c_int32, C.c_int32, C.c_int32, vp,
                                              C.c_double, C.c_int32, C.c_double, C.c_int32, C.c_int32,
                                              vp, vp, vp, C.c_uint64, C.c_int32] + [vp] * 8)
+    lib.omg_closed_loop_step_free.argtypes = ([C.c_int32] * 5 + [vp] + [C.c_int32] * 4 + [vp, C.c_int32, C.c_int32,
+                                              vp, vp, C.c_double, C.c_int32, C.c_double, C.c_int32,
+                                              vp, vp, vp, C.c_uint64, C.c_int32] + [vp] * 8)
     lib.omg_shift_free_batch.argtypes = [vp, C.c_int32, vp, C.c_int32, C.c_double, vp, C.c_int32] + [vp] * 6
     lib.omg_eval_batch.argtypes = [C.c_int32, C.c_int32, vp, C.c_int32] + [vp] * 5 + [C.c_int32, vp, vp, C.c_int32,
                                                                                     vp, vp]
@@ -817,5 +820,57 @@ def closed_loop_step(model, X, L, R0, R1, sample_time, plant_x, plant_u, out, st
         R = np.ascontiguousarray(np.concatenate(rows))
         rc = lib.omg_closed_loop_step_der(mid, B, ns, ni, X.shape[1], X.data_ptr(), L, R0.shape[0] - 1,
                                           R.shape[0], R.ctypes.data, *rest)
+    if rc != 0:
+        raise RuntimeError('libomgb200: %s' % lib.omg_last_error().decode())
+
+
+def closed_loop_step_free(model, X, block, t_index, n_der, n_samp, sample_time, plant_x, plant_u, out, step,
+                          seed=0, time_constant=None, disturbance=None, stream=None):
+    """closed_loop_step with a free motion time (omg_closed_loop_step_free): instance b samples its
+    plan at s * sample_time / T_b, T_b = X[b, t_index], for s = 0..n_samp[b] (0 = b is left alone).
+    block = (offset, len_basis, n_columns, degree, knots) of the spline block whose first columns
+    are the input splines (spline_blocks(father, vehicle)[0]); n_der: derivative rows the model
+    reads (2 to 4).  n_samp: host int array [B].  disturbance: (filt, mean, stdev, n_traj, scratch)
+    with n_traj a host int array [B] (0 = no disturbance for that instance) and scratch a float64
+    tensor of at least B * n_input * (max(n_traj) + 24) elements (None = off).  Every other
+    argument is closed_loop_step's."""
+    lib = load_library()
+    mid = ODE_MODELS[model] if isinstance(model, str) else int(model)
+    tensors = (X, plant_x, plant_u) + tuple(out)
+    B, ns = plant_x.shape
+    ni = plant_u.shape[1]
+    n_samp = np.ascontiguousarray(n_samp, dtype=np.int32).reshape(-1)
+    if n_samp.size != B:
+        raise ValueError('n_samp must hold one count per instance')
+    d = disturbance is not None
+    if d:
+        filt, mean, stdev, n_traj, scratch = disturbance
+        tensors += (scratch,)
+        n_traj = np.ascontiguousarray(n_traj, dtype=np.int32).reshape(-1)
+        if n_traj.size != B:
+            raise ValueError('n_traj must hold one count per instance')
+        if scratch.numel() < B * ni * (int(n_traj.max(initial=0)) + 24):
+            raise ValueError('disturbance scratch too small')
+        filt, mean, stdev = (np.ascontiguousarray(a, dtype=np.float64) for a in (filt, mean, stdev))
+        if filt.size != 11 or mean.size != ni or stdev.size != ni:
+            raise ValueError('disturbance filter / mean / stdev sizes')
+    on_gpu = _check_device_tensors(tensors, lib)
+    if X.dim() != 2 or X.shape[0] != B:
+        raise ValueError('X must be [B, n] with the batch of plant_x')
+    for t, shape in zip(out, ((B, ns), (B, ni), (B, ns), (B, ni))):
+        if tuple(t.shape) != shape:
+            raise ValueError('output tensor shapes do not match the plant state / input')
+    off, L, nc, degree, knots = block
+    knots = np.ascontiguousarray(knots, dtype=np.float64).reshape(-1)
+    if knots.size != L + degree + 1:
+        raise ValueError('a block of length %d and degree %d needs %d knots, got %d'
+                         % (L, degree, L + degree + 1, knots.size))
+    rc = lib.omg_closed_loop_step_free(
+        mid, B, ns, ni, X.shape[1], X.data_ptr(), int(off), int(L), int(nc), int(degree), knots.ctypes.data,
+        int(t_index), int(n_der), n_samp.ctypes.data, n_traj.ctypes.data if d else None, float(sample_time),
+        int(time_constant is not None), float(time_constant) if time_constant is not None else 0., int(d),
+        filt.ctypes.data if d else None, mean.ctypes.data if d else None, stdev.ctypes.data if d else None,
+        int(seed) & 0xFFFFFFFFFFFFFFFF, int(step), plant_x.data_ptr(), plant_u.data_ptr(),
+        *[t.data_ptr() for t in out], scratch.data_ptr() if d else None, _stream_handle(on_gpu, X.device, stream))
     if rc != 0:
         raise RuntimeError('libomgb200: %s' % lib.omg_last_error().decode())

@@ -1,6 +1,6 @@
 """Cost of the batched MPC loop with a free motion time (execution/batch_mpc.py, FreeTPoint2point).
 
-    python tools/freet_mpc_bench.py [--steps 40] [--out DIR]
+    python tools/freet_mpc_bench.py [--steps 40] [--closed] [--out DIR]
 
 Two workloads at 0.5 s updates: config_freeT with a jittered batch of 1024 (jitter 0.1) and
 config_dubins_freeT (init_v_til = 0.3) with a jittered batch of 256.  Each runs until every
@@ -9,7 +9,11 @@ step (closed by a device synchronise), the solve time (CUDA events around the so
 time of the warm-start (omg_shift_free_batch) and prediction (omg_eval_batch) launches alone (CUDA
 events around each call), and the number of active instances.  For comparison, the host path of
 the warm start, shift_spline on every shifted block of each active instance (what the sequential
-loop does per instance), is timed on the instances and motion times of the second step.  The card's
+loop does per instance), is timed on the instances and motion times of the second step.  With
+--closed the loops run through the vehicle's own dynamics at the reference's vehicle defaults
+(ideal_update and ideal_prediction off) with the first-order lag (time constant 0.1) and the input
+disturbance (fc 0.01, stdev 0.05), and the plant step (omg_closed_loop_step_free) is timed like the
+other launches; the host's shift_spline is not timed then.  The card's
 name and power limit are read in the same call.  Needs a CUDA device; prints one JSON line and
 writes it to DIR/freet_mpc_bench.json when --out is given."""
 import argparse
@@ -26,6 +30,8 @@ sys.path.insert(0, ROOT)
 
 WORKLOADS = [('config_freeT', 1024, {}), ('config_dubins_freeT', 256, {'init_v_til': 0.3})]
 DT = 0.5
+CLOSED = {'ideal_update': False, 'ideal_prediction': False, '1storder_delay': True, 'time_constant': 0.1,
+          'input_disturbance': {'fc': 0.01, 'stdev': 0.05 * np.ones(2)}}
 
 
 def card():
@@ -60,24 +66,28 @@ def host_shift_ms(bat, X, T, n_max=64):
     return 1e3 * (time.perf_counter() - t0) / len(idx)
 
 
-def one_run(name, batch, kw, steps):
+def one_run(name, batch, kw, steps, closed=False):
     import torch
     from omg_tools_b200 import scenarios as sc
     from omg_tools_b200.execution.batch_mpc import BatchMPC
     from omg_tools_b200.solver import b200
-    bat = BatchMPC(getattr(sc, name)(**kw), batch=batch, update_time=DT, seed=1, jitter=0.1)
-    ev = {'solve': [], 'shift': [], 'eval': []}
+    pr = getattr(sc, name)(**kw)
+    if closed:
+        pr.vehicles[0].set_options(CLOSED)
+    bat = BatchMPC(pr, batch=batch, update_time=DT, seed=1, jitter=0.1)
+    ev = {'solve': [], 'shift': [], 'eval': [], 'plant': []}
     bat.solver.solve_batch_device = _timed(ev['solve'], bat.solver.solve_batch_device)
     bat.solver.shift_free_batch_device = _timed(ev['shift'], bat.solver.shift_free_batch_device)
-    eval_fn = b200.eval_batch
+    eval_fn, plant_fn = b200.eval_batch, b200.closed_loop_step_free
     b200.eval_batch = _timed(ev['eval'], eval_fn)
+    b200.closed_loop_step_free = _timed(ev['plant'], plant_fn)
     rows = []
     host_ms = None
     try:
         for k in range(steps):
             if not bat.active.any():
                 break
-            if k == 1:
+            if k == 1 and not closed:
                 host_ms = host_shift_ms(bat, bat.X.cpu().numpy(), bat.X[:, bat.t_index].cpu().numpy())
             n_act = int(bat.active.sum())
             for v in ev.values():
@@ -89,15 +99,15 @@ def one_run(name, batch, kw, steps):
             wall = 1e3 * (time.perf_counter() - t0)
             ms = {key: sum(a.elapsed_time(b) for a, b in v) for key, v in ev.items()}
             rows.append({'active': n_act, 'wall_ms': wall, 'solve_ms': ms['solve'], 'shift_ms': ms['shift'],
-                         'eval_ms': ms['eval']})
+                         'eval_ms': ms['eval'], 'plant_ms': ms['plant']})
     finally:
-        b200.eval_batch = eval_fn
+        b200.eval_batch, b200.closed_loop_step_free = eval_fn, plant_fn
     fail = int(sum((s > 0).sum() for s in bat.history['status']))
     med = lambda key: float(np.median([r[key] for r in rows[1:]]))     # (step 0: cold start)
-    return {'scenario': name, 'batch': batch, 'steps': len(rows), 'stopped': int((~bat.active).sum()),
+    return {'scenario': name, 'batch': batch, 'closed': closed, 'steps': len(rows), 'stopped': int((~bat.active).sum()),
             'failed_solves': fail, 'active_per_step': [r['active'] for r in rows],
             'wall_ms_median': med('wall_ms'), 'solve_ms_median': med('solve_ms'),
-            'shift_ms_median': med('shift_ms'), 'eval_ms_median': med('eval_ms'),
+            'shift_ms_median': med('shift_ms'), 'eval_ms_median': med('eval_ms'), 'plant_ms_median': med('plant_ms'),
             'host_shift_spline_ms_per_instance': host_ms,
             'host_shift_spline_ms_per_step_at_batch': host_ms * batch if host_ms else None,
             'per_step': rows}
@@ -106,6 +116,7 @@ def one_run(name, batch, kw, steps):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--steps', type=int, default=40)
+    ap.add_argument('--closed', action='store_true', help='closed loop with lag and disturbance')
     ap.add_argument('--out', default=None)
     a = ap.parse_args()
     import torch
@@ -113,12 +124,13 @@ def main():
         raise SystemExit('freet_mpc_bench.py needs a CUDA device')
     res = {'card': card(), 'device': torch.cuda.get_device_name(0), 'update_time': DT, 'runs': []}
     for name, batch, kw in WORKLOADS:
-        res['runs'].append(one_run(name, batch, kw, a.steps))
+        res['runs'].append(one_run(name, batch, kw, a.steps, a.closed))
     line = json.dumps(res)
     print(line)
     if a.out:
         os.makedirs(a.out, exist_ok=True)
-        with open(os.path.join(a.out, 'freet_mpc_bench.json'), 'w') as f:
+        fn = 'freet_mpc_bench_closed.json' if a.closed else 'freet_mpc_bench.json'
+        with open(os.path.join(a.out, fn), 'w') as f:
             f.write(line + '\n')
 
 
