@@ -10,10 +10,11 @@
 //     supernode levels + one dense root of 36 columns.
 //       - SUPERNODES: paths of the elimination tree of up to SP_SNW columns with the structure
 //         of their last column (few explicit zeros), one level step each:
-//         GATHER, left-looking, one thread per stored entry: one record per (entry, source
-//         supernode) -- byte offsets of the two rows in the supernode's first column + its table
-//         entry -- contributes  v -= sum_t A_it * rd_t * A_jt  over the supernode's columns
-//         (unscaled columns A = L D, rd = 1/d: the pivot signs come with d);
+//         GATHER, left-looking, one thread per column segment (SP_GQ consecutive stored entries
+//         of one column): one record per (segment, source supernode) -- byte offsets of the
+//         shared row j and of each entry's row i in the supernode's first column + its table
+//         entry -- contributes  v -= sum_t A_it * rd_t * A_jt  over the supernode's columns to
+//         every entry it reaches (unscaled columns A = L D, rd = 1/d: the pivot signs come with d);
 //         PANEL: one task per panel row; every task factorises the w x w diagonal block for
 //         itself (identical arithmetic) and finishes its row -- no block barrier inside;
 //       - the dense root (the final chain of the elimination tree, <= 40 columns): right-looking
@@ -66,11 +67,12 @@ struct SpTab {
   int Lsz, zslot, R0, nr, n_lev, root0, n_rootent;
   int neg_lev;                     // levels < neg_lev hold only variables no equality row touches: a negative
                                    //   pivot there already decides the inertia test (see SP_CHECK)
-  // factorisation levels (+ the gather into the root as level n_lev): slices of 32 entries
+  // factorisation levels (+ the gather into the root as level n_lev): slices of 32 column segments
   const int* lev_ptr;              // [n_lev+2] slice ranges
-  const uint4* fdesc;              // per slice lane: {entry word, pair offset (uint4 units), n4, 0}
-                                   //   entry word: lidx | col<<13 | isdiag<<24 | eq-pivot<<25 (0xffffffff idle)
-  const uint4* fpair;              // 2 pairs per uint4, [slice][k2][lane]; pair = {a8 | b8<<16, k8}: byte offsets into LK / rd
+  const uint4* fdesc;              // per slice lane: {segment word, record offset (uint4 units), records, 0}
+                                   //   segment word: lidx of its first entry | col<<13 | isdiag<<24 | eq-pivot<<25 |
+                                   //   (entries - 1)<<26 (0xffffffff idle); isdiag / eq-pivot: of the first entry
+  const uint4* fpair;              // segment records (SP_SEG), [slice][k][lane]
   const unsigned* root_ch;         // [SP_RCH * nt] row chunk of a thread: i | k0<<6 | cnt<<12 | eq-pivot<<16
                                    //   (root-local row i (nr = rhs), columns k0 .. k0+cnt-1; 0: none)
   const uint4* sntab; int n_sn;    // per supernode (+ a dummy): {d1 | d2<<16, d3 | r0<<16, r1 | r2<<16, r3}: byte distance from a
@@ -281,24 +283,38 @@ SP_COLD double sp_eval_range(const PTerm* t, int lo, int hi, const double* V, co
       return;                                                                                 \
     }                                                                                         \
   }
-// pair record (8 bytes): byte offsets a8 | b8<<16 into LK, k8 into rd -- no index arithmetic
 #define SP_LDB(base, off) (*reinterpret_cast<const double*>(reinterpret_cast<const char*>(base) + (off)))
-// (record: byte offsets of the two rows' entries in the source supernode's first column, byte
-// offset of the supernode's table entry; up to four columns contribute)
-#define SP_PAIR(lo, hi)                                                                        \
+// segment record (16 bytes): {j8 | table entry<<16, i8 of entries 0, 1 | 2, 3 | 4, 5 as 16-bit
+// halves}: byte offsets into LK of the rows' entries in the source supernode's first column (0:
+// the source does not reach that entry), byte offset of the supernode's table entry.  The table
+// entry, A_j. and rd are loaded once; entry q sums  v -= (A_it * rd_t) * A_jt  over the up to four
+// columns t, columns 0 and 2 into v0[q], 1 and 3 into v1[q] -- the products, their order and the
+// accumulators of one record per (entry, source).
+#ifndef SP_GQ
+#define SP_GQ 2                  // entries per segment
+#endif
+#define SP_SEG(rc)                                                                             \
   {                                                                                           \
-    const uint4 st_ = *reinterpret_cast<const uint4*>(sntb + (hi));                           \
-    const char* pa_ = reinterpret_cast<const char*>(LK) + ((lo) & 0xffffu);                   \
-    const char* pb_ = reinterpret_cast<const char*>(LK) + ((lo) >> 16);                       \
-    v0 -= SP_LDB(pa_, 0) * SP_LDB(rd, st_.y >> 16) * SP_LDB(pb_, 0);                          \
-    v1 -= SP_LDB(pa_, st_.x & 0xffffu) * SP_LDB(rd, st_.z & 0xffffu) * SP_LDB(pb_, st_.x & 0xffffu); \
-    v0 -= SP_LDB(pa_, st_.x >> 16) * SP_LDB(rd, st_.z >> 16) * SP_LDB(pb_, st_.x >> 16);      \
-    v1 -= SP_LDB(pa_, st_.y & 0xffffu) * SP_LDB(rd, st_.w) * SP_LDB(pb_, st_.y & 0xffffu);    \
+    const uint4 st_ = *reinterpret_cast<const uint4*>(sntb + ((rc).x >> 16));                 \
+    const char* pb_ = reinterpret_cast<const char*>(LK) + ((rc).x & 0xffffu);                 \
+    const double b0_ = SP_LDB(pb_, 0), b1_ = SP_LDB(pb_, st_.x & 0xffffu),                    \
+                 b2_ = SP_LDB(pb_, st_.x >> 16), b3_ = SP_LDB(pb_, st_.y & 0xffffu);          \
+    const double r0_ = SP_LDB(rd, st_.y >> 16), r1_ = SP_LDB(rd, st_.z & 0xffffu),            \
+                 r2_ = SP_LDB(rd, st_.z >> 16), r3_ = SP_LDB(rd, st_.w);                      \
+    _Pragma("unroll") for (int q_ = 0; q_ < SP_GQ; ++q_) {                                    \
+      const unsigned o_ = (((q_ < 2) ? (rc).y : (q_ < 4) ? (rc).z : (rc).w) >> (16 * (q_ & 1))) & 0xffffu; \
+      if (o_) {                                                                               \
+        const char* pa_ = reinterpret_cast<const char*>(LK) + o_;                             \
+        v0[q_] -= SP_LDB(pa_, 0) * r0_ * b0_;                                                 \
+        v1[q_] -= SP_LDB(pa_, st_.x & 0xffffu) * r1_ * b1_;                                   \
+        v0[q_] -= SP_LDB(pa_, st_.x >> 16) * r2_ * b2_;                                       \
+        v1[q_] -= SP_LDB(pa_, st_.y & 0xffffu) * r3_ * b3_;                                   \
+      }                                                                                       \
+    }                                                                                         \
   }
-#define SP_PAIR4(pc) { SP_PAIR((pc).x, (pc).y) SP_PAIR((pc).z, (pc).w) }
-// descriptor of slice sl (idle if the level has no slice for this warp) / its first 16 pairs
+// descriptor of slice sl (idle if the level has no slice for this warp) / its first records
 #define SP_FDESC(d, sl, s_end) { (d) = make_uint4(0xffffffffu, 0u, 0u, 0u); if ((sl) < (s_end)) (d) = __ldg(P.fdesc + (sl) * 32 + lane); }
-#define SP_NPF 2                 // uint4 words (2 pairs each) of every entry fetched one level ahead
+#define SP_NPF 2                 // records of every segment fetched one level ahead (= records per loop step)
 #define SP_FPAIRS(p, d) { const uint4* q_ = P.fpair + (d).y;                                   \
     _Pragma("unroll") for (int w_ = 0; w_ < SP_NPF; ++w_) if ((d).z > (unsigned)w_) (p)[w_] = __ldg(q_ + 32 * w_); }
 
@@ -348,30 +364,36 @@ __device__ __forceinline__ void sp_factor(const DevTab& T, const SpTab& P, const
       const uint4 d = dA;
       const unsigned e = d.x;
       const int li = (e == 0xffffffffu) ? P.zslot : (int)(e & 0x1fffu);
-      const int n4 = (int)d.z;
-      double v0 = LK[li], v1 = 0.0;
-      // one loop body over the words in list order: the prefetched words first, then groups of
-      // four; the next group's four loads are in flight while the current one is summed
-      uint4 c[4];
+      const int cnt = (e == 0xffffffffu) ? 0 : (int)((e >> 26) & 7u) + 1;
+      const int nk = (int)d.z;
+      double v0[SP_GQ], v1[SP_GQ];
 #pragma unroll
-      for (int t = 0; t < 4; ++t) c[t] = (t < SP_NPF) ? pA[t < SP_NPF ? t : 0] : make_uint4(0u, 0u, 0u, 0u);
-      int nc = (n4 < SP_NPF) ? n4 : SP_NPF;
-      uint4 r[4] = {};                   // words past the list are copied to c but never summed
-      for (int k = SP_NPF;; k += 4) {
+      for (int q = 0; q < SP_GQ; ++q) { v0[q] = LK[li + q]; v1[q] = 0.0; }
+      // one loop body over the records in source order: the prefetched records first, then groups
+      // of SP_NPF; the next group's loads are in flight while the current one is summed
+      uint4 c[SP_NPF];
+#pragma unroll
+      for (int t = 0; t < SP_NPF; ++t) c[t] = pA[t];
+      int nc = (nk < SP_NPF) ? nk : SP_NPF;
+      uint4 r[SP_NPF] = {};              // records past the list are copied to c but never summed
+      for (int k = SP_NPF;; k += SP_NPF) {
         const uint4* q_ = P.fpair + d.y + k * 32;
 #pragma unroll
-        for (int t = 0; t < 4; ++t) if (k + t < n4) r[t] = __ldg(q_ + t * 32);
+        for (int t = 0; t < SP_NPF; ++t) if (k + t < nk) r[t] = __ldg(q_ + t * 32);
 #pragma unroll
-        for (int t = 0; t < 4; ++t) if (t < nc) SP_PAIR4(c[t])
-        if (k >= n4) break;
-        nc = (n4 - k < 4) ? n4 - k : 4;
+        for (int t = 0; t < SP_NPF; ++t) if (t < nc) SP_SEG(c[t])
+        if (k >= nk) break;
+        nc = (nk - k < SP_NPF) ? nk - k : SP_NPF;
 #pragma unroll
-        for (int t = 0; t < 4; ++t) c[t] = r[t];
+        for (int t = 0; t < SP_NPF; ++t) c[t] = r[t];
       }
-      const double v = v0 + v1;
-      if (e != 0xffffffffu) {
-        LK[li] = v;
-        if (e & (1u << 24)) { const int j = (e >> 13) & 0x7ffu; SP_PIVOT(j, v, (e & (1u << 25)) != 0u) }
+#pragma unroll
+      for (int q = 0; q < SP_GQ; ++q) {
+        if (q < cnt) {
+          const double v = v0[q] + v1[q];
+          LK[li + q] = v;
+          if (q == 0 && (e & (1u << 24))) { const int j = (e >> 13) & 0x7ffu; SP_PIVOT(j, v, (e & (1u << 25)) != 0u) }
+        }
       }
     }
     if (lv1 != lv) {                                        // the level's last step

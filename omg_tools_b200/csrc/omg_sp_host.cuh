@@ -258,12 +258,13 @@ static bool sp_setup(omg_problem* h, const omg_tables* tb, const cudaDeviceProp&
 
 
   // ---- pair lists of the left-looking gather -----------------------------------------
-  // One record per (target entry, source SUPERNODE): with the rows i, j of the target among the
+  // One pair per (target entry, source SUPERNODE): with the rows i, j of the target among the
   // rows R below the supernode's block, the w columns contribute
   //     sum_t x_it x_jt / d_t        (padded entries are zero, so every column may be summed).
-  // Record = {byte offset of (i, first column) | of (j, first column) << 16, byte offset of the
+  // Pair = {byte offset of (i, first column) | of (j, first column) << 16, byte offset of the
   // supernode's table entry}; the table entry holds the byte distance from a row's entry in the
-  // first column to its entry in column t, and where 1/d_t lives (a zero for t >= w).
+  // first column to its entry in column t, and where 1/d_t lives (a zero for t >= w).  The
+  // segments below merge the pairs of neighbouring entries into the kernel's records.
   std::vector<std::vector<uint2>> plist(Y.Lsize);
   std::vector<uint4> sntab;
   for (int c0 = 0; c0 < R0; ++c0) {
@@ -296,46 +297,82 @@ static bool sp_setup(omg_problem* h, const omg_tables* tb, const cudaDeviceProp&
   if (sntab.size() * 16u >= 65536u) { *why = "too many supernodes"; return false; }
   P.n_sn = (int)sntab.size();
   P.sntab = upload(h, sntab.data(), sntab.size(), &ok);
-  const uint2 padpair = make_uint2(((unsigned)P.zslot * 8u) | (((unsigned)P.zslot * 8u) << 16), sn_dummy);
   std::vector<char> is_eq_pos(N, 0);          // permuted index -> pivot of an equality row
   for (int k = 0; k < n_eq; ++k) is_eq_pos[Y.pos[n + k]] = 1;
+  // ---- segments of the gather ----------------------------------------------------------------
+  // A segment is up to SP_GQ consecutive stored entries of one column: all of a level column's
+  // entries, and on the root the runs of entries with a non-empty list.  Its entries share the row
+  // j of every source, so ONE 16-byte record per (segment, source) serves all of them: {byte offset
+  // of (j, first column) | table entry << 16, then the byte offsets of (i_q, first column) as 16-bit
+  // halves, 0 where the source does not reach entry q}.  The kernel unpacks the table entry and
+  // loads A_j. and rd once per record.  Records are the union of the entries' sources in ascending
+  // supernode order, so every entry receives its contributions in the order of its pair list.
+  static_assert(SP_GQ >= 1 && SP_GQ <= 6, "entry offsets: six 16-bit halves of a record");
+  const uint4 padrec = make_uint4(((unsigned)P.zslot * 8u) | (sn_dummy << 16), 0u, 0u, 0u);
   std::vector<int> lev_ptr;
   std::vector<uint4> fdesc, fpair;
+  size_t pair_slots = 0;                      // record slots of one record per (entry, source), 2 per uint4
+  int n_seg = 0, max_seg_src = 0, seg_mismatch = 0;
   for (int lv = 0; lv <= Y.n_lev; ++lv) {
-    std::vector<unsigned> ents;        // entry words
-    std::vector<int> lidx;
-    if (lv < Y.n_lev) {
-      for (int j = 0; j < R0; ++j) if (Y.lev[j] == lv)
-        for (int e = Y.colptr[j]; e < Y.colptr[j + 1]; ++e) {
-          lidx.push_back(e);
-          const bool piv = (e == Y.colptr[j]) && Y.sn_w[j] == 1;    // wider supernodes: pivots in the panel step
-          if (piv && is_eq_pos[j]) ++eq_lev;
-          ents.push_back((unsigned)e | ((unsigned)j << 13) | (piv ? (1u << 24) : 0u) |
-                         ((piv && is_eq_pos[j]) ? (1u << 25) : 0u));
+    std::vector<unsigned> words;              // segment words
+    std::vector<std::vector<uint4>> recs;     // records of each segment
+    std::vector<size_t> lens;                 // list length of each entry the level gathers
+    const bool root = (lv == Y.n_lev);
+    for (int j = root ? R0 : 0; j < (root ? N : R0); ++j) {
+      if (!root && Y.lev[j] != lv) continue;
+      for (int e0 = Y.colptr[j]; e0 < Y.colptr[j + 1];) {
+        if (root && plist[e0].empty()) { ++e0; continue; }
+        int cnt = 0;
+        while (cnt < SP_GQ && e0 + cnt < Y.colptr[j + 1] && !(root && plist[e0 + cnt].empty())) ++cnt;
+        std::map<unsigned, uint4> src;        // table entry -> record
+        for (int q = 0; q < cnt; ++q) {
+          lens.push_back(plist[e0 + q].size());
+          for (const uint2& p : plist[e0 + q]) {
+            uint4& r = src.emplace(p.y, make_uint4((p.x >> 16) | (p.y << 16), 0u, 0u, 0u)).first->second;
+            (&r.y)[q / 2] |= (p.x & 0xffffu) << (16 * (q % 2));
+          }
         }
-    } else {
-      for (int e = Y.colptr[R0]; e < Y.Lsize; ++e) if (!plist[e].empty()) { lidx.push_back(e); ents.push_back((unsigned)e); }
+        recs.emplace_back();
+        for (const auto& kv : src) recs.back().push_back(kv.second);
+        // what the kernel reads back: entry q's (i, j, table entry) in record order = its pair list
+        for (int q = 0; q < cnt; ++q) {
+          std::vector<uint2> back;
+          for (const uint4& r : recs.back()) {
+            const unsigned o = ((&r.y)[q / 2] >> (16 * (q % 2))) & 0xffffu;
+            if (o) back.push_back(make_uint2(o | ((r.x & 0xffffu) << 16), r.x >> 16));
+          }
+          const std::vector<uint2>& pl = plist[e0 + q];
+          bool same = back.size() == pl.size();
+          for (size_t k = 0; same && k < pl.size(); ++k) same = back[k].x == pl[k].x && back[k].y == pl[k].y;
+          if (!same) ++seg_mismatch;
+        }
+        const bool piv = !root && e0 == Y.colptr[j] && Y.sn_w[j] == 1;   // wider supernodes: pivots in the panel step
+        if (piv && is_eq_pos[j]) ++eq_lev;
+        words.push_back((unsigned)e0 | (root ? 0u : (unsigned)j << 13) | (piv ? (1u << 24) : 0u) |
+                        ((piv && is_eq_pos[j]) ? (1u << 25) : 0u) | ((unsigned)(cnt - 1) << 26));
+        e0 += cnt;
+      }
     }
-    std::vector<int> ord(ents.size());
+    // the per-entry layout (slices of 32 entries, lists in words of two pairs) that the structure
+    // line's pairs= and max-slices= keep counting
+    std::stable_sort(lens.begin(), lens.end(), std::greater<size_t>());
+    for (size_t q0 = 0; q0 < lens.size(); q0 += 32) pair_slots += (lens[q0] + 1) / 2 * 64;
+    max_slices = std::max(max_slices, (int)((lens.size() + 31) / 32));
+    n_seg += (int)recs.size();
+    std::vector<int> ord(recs.size());
     for (size_t q = 0; q < ord.size(); ++q) ord[q] = (int)q;
-    std::stable_sort(ord.begin(), ord.end(), [&](int a, int b) { return plist[lidx[a]].size() > plist[lidx[b]].size(); });
-    max_slices = std::max(max_slices, (int)((ord.size() + 31) / 32));
+    std::stable_sort(ord.begin(), ord.end(), [&](int a, int b) { return recs[a].size() > recs[b].size(); });
     lev_ptr.push_back((int)(fdesc.size() / 32));
     for (size_t q0 = 0; q0 < ord.size(); q0 += 32) {
-      size_t mx = 0;
-      for (size_t q = q0; q < std::min(q0 + 32, ord.size()); ++q) mx = std::max(mx, plist[lidx[ord[q]]].size());
-      const unsigned n4 = (unsigned)((mx + 1) / 2);          // uint4 words of 2 pairs
+      const unsigned nk = (unsigned)recs[ord[q0]].size();    // records per lane
+      max_seg_src = std::max(max_seg_src, (int)nk);
       const unsigned pbase = (unsigned)fpair.size();
-      fpair.resize(fpair.size() + (size_t)n4 * 32, make_uint4(padpair.x, padpair.y, padpair.x, padpair.y));
+      fpair.resize(fpair.size() + (size_t)nk * 32, padrec);
       for (int l = 0; l < 32; ++l) {
         const size_t q = q0 + l;
-        if (q >= ord.size()) { fdesc.push_back(make_uint4(0xffffffffu, pbase + l, n4, 0u)); continue; }
-        const std::vector<uint2>& pl = plist[lidx[ord[q]]];
-        fdesc.push_back(make_uint4(ents[ord[q]], pbase + l, n4, 0u));
-        for (size_t k = 0; k < pl.size(); ++k) {
-          uint4& w = fpair[pbase + (k / 2) * 32 + l];
-          if (k % 2 == 0) { w.x = pl[k].x; w.y = pl[k].y; } else { w.z = pl[k].x; w.w = pl[k].y; }
-        }
+        if (q >= ord.size()) { fdesc.push_back(make_uint4(0xffffffffu, pbase + l, nk, 0u)); continue; }
+        fdesc.push_back(make_uint4(words[ord[q]], pbase + l, nk, 0u));
+        for (size_t k = 0; k < recs[ord[q]].size(); ++k) fpair[pbase + k * 32 + l] = recs[ord[q]][k];
       }
     }
   }
@@ -646,7 +683,7 @@ static bool sp_setup(omg_problem* h, const omg_tables* tb, const cudaDeviceProp&
   h->sp_dscr_stride = goff + 8;
   h->sp_info = "sparse LDL^T: N=" + std::to_string(N) + " nnz(L)=" + std::to_string(Y.Lsize) +
                h->sp_info_extra + " levels=" + std::to_string(Y.n_lev) + " (early-reject " + std::to_string(P.neg_lev) + ")" + " root=" + std::to_string(nr) +
-               " pairs=" + std::to_string(fpair.size() * 2) + " nt=" + std::to_string(nt) +
+               " pairs=" + std::to_string(pair_slots) + " nt=" + std::to_string(nt) +
                " ctas/SM=" + std::to_string(occ) + " smem=" + std::to_string(h->sp_smem_bytes) +
                " scratch/iter=" + std::to_string(touched);
   auto kv = [&](const char* k, int v) { h->sp_info += std::string(" ") + k + "=" + std::to_string(v); };
@@ -657,5 +694,7 @@ static bool sp_setup(omg_problem* h, const omg_tables* tb, const cudaDeviceProp&
   kv("max-gather", max_gather); kv("max-nq", max_nq); kv("max-slices", max_slices);
   kv("max-block-rows", max_blk); kv("max-panel-rounds", max_prounds); kv("max-back-rounds", max_brounds);
   kv("root-mod4", nr % 4);
+  kv("segments", n_seg); kv("seg-records", (int)fpair.size()); kv("max-seg-sources", max_seg_src);
+  kv("seg-mismatch", seg_mismatch);
   return true;
 }
