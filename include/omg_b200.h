@@ -360,6 +360,27 @@ int omg_closed_loop_step_der(int32_t model, int32_t B, int32_t n_state, int32_t 
                              const double* plant_u, double* plant_x_next, double* plant_u_next,
                              double* pred_x, double* pred_u, double* scratch, void* stream);
 
+/* omg_closed_loop_step_der for a fleet of n_veh vehicles of one model and one spline basis in
+ * each row of x (a multi-vehicle problem, reference Problem.simulate / predict looping over
+ * self.vehicles, problem.py:187-192): vehicle v's n_input input splines are the columns of
+ * length L at x[b, veh_off[v] + c*L].  HOST int32 veh_off [n_veh].  DEVICE plant_x, plant_u and
+ * the four outputs are [B x n_veh x n_state | n_input]; scratch holds
+ * B x n_veh x n_input x (n_traj + 24) doubles (disturb only).  One block of 32 threads per
+ * (instance, vehicle).  The noise of vehicle v's input j is keyed by (seed, step, b, v*n_input + j,
+ * sample pair): vehicle 0 draws what omg_closed_loop_step_der draws, and a realisation does not
+ * depend on the batch size.  With n_veh = 1 and veh_off = {0} the outputs are
+ * omg_closed_loop_step_der's, bit for bit (that entry point launches the same kernel).  Rejected
+ * with a message: everything omg_closed_loop_step_der rejects, n_veh < 1, a null veh_off, and an
+ * offset < 0 or with veh_off[v] + n_input*L > n. */
+int omg_closed_loop_step_fleet(int32_t model, int32_t B, int32_t n_veh, int32_t n_state, int32_t n_input,
+                               int32_t n, const double* x, const int32_t* veh_off, int32_t L,
+                               int32_t n_samp, int32_t n_der, const double* R, double sample_time,
+                               int32_t lag, double time_constant, int32_t disturb, int32_t n_traj,
+                               const double* filt, const double* mean, const double* stdev,
+                               uint64_t seed, int32_t step, const double* plant_x,
+                               const double* plant_u, double* plant_x_next, double* plant_u_next,
+                               double* pred_x, double* pred_u, double* scratch, void* stream);
+
 /* omg_closed_loop_step_der with a free motion time (reference FreeTPoint2point.store / simulate,
  * point2point.py:313-346, on Vehicle.store / predict / simulate): every instance samples its own
  * plan on its own time axis, so no basis row is shared and the rows are built on the device.

@@ -1394,9 +1394,11 @@ __device__ __forceinline__ void omg_cl_input_map(int model, int ni, const double
 // filtfilt(butter(3, fc)): odd extension by 12, forward and backward passes of the transposed
 // direct form from zi * (first value); only samples 0..n_samp are kept.
 // filt = {b0..b3, a0..a3 (a0 = 1), zi0..zi2}; scratch holds one forward pass per series, `stride`
-// doubles apart (at least n_traj + 24).  D, A: [n_samp+1][ni] of shared memory.  The noise is
-// keyed by (seed, step, b, signal, pair).
-__device__ void omg_cl_tail(int b, int ode, int ns, int ni, int n_samp, double dt, int lag, double tau,
+// doubles apart (at least n_traj + 24).  D, A: [n_samp+1][ni] of shared memory.  p indexes the
+// plant arrays ([p][ns], [p][ni]) and the scratch series; the noise of input j is keyed by (seed,
+// step, b, sig0 + j, pair), so that the vehicles of a fleet (p = b*n_veh + v, sig0 = v*ni) draw
+// their own series and vehicle 0 draws what a single vehicle draws.
+__device__ void omg_cl_tail(int b, int p, int sig0, int ode, int ns, int ni, int n_samp, double dt, int lag, double tau,
                             int disturb, int n_traj, const double* __restrict__ filt,
                             const double* __restrict__ mean, const double* __restrict__ stdev, uint64_t seed,
                             int step, const double* plant_x, const double* plant_u, double* plant_x_next,
@@ -1405,13 +1407,13 @@ __device__ void omg_cl_tail(int b, int ode, int ns, int ni, int n_samp, double d
   const int ts = n_samp + 1;
   if (disturb && (int)threadIdx.x < ni) {
     const int j = threadIdx.x, N = n_traj + 2 * OMG_CL_PAD;
-    double* e = scratch + ((size_t)b * ni + j) * stride;
+    double* e = scratch + ((size_t)p * ni + j) * stride;
     double* w = e + OMG_CL_PAD;                     // white noise at 0..n_traj-1
-    for (int p = 0; 2 * p < n_traj; ++p) {
+    for (int q = 0; 2 * q < n_traj; ++q) {
       double z0, z1;
-      omg_normal_pair(seed, step, b, j, p, &z0, &z1);
-      w[2 * p] = mean[j] + stdev[j] * z0;
-      if (2 * p + 1 < n_traj) w[2 * p + 1] = mean[j] + stdev[j] * z1;
+      omg_normal_pair(seed, step, b, sig0 + j, q, &z0, &z1);
+      w[2 * q] = mean[j] + stdev[j] * z0;
+      if (2 * q + 1 < n_traj) w[2 * q + 1] = mean[j] + stdev[j] * z1;
     }
     for (int i = 1; i <= OMG_CL_PAD; ++i) {         // odd extension (scipy odd_ext)
       e[OMG_CL_PAD - i] = 2.0 * w[0] - w[i];
@@ -1437,7 +1439,7 @@ __device__ void omg_cl_tail(int b, int ode, int ns, int ni, int n_samp, double d
          k4[OMG_ODE_MAX_STATE], y[OMG_ODE_MAX_STATE], um[OMG_CL_MAX_INPUT];
   // read before the barrier: the outputs may overwrite the plant state in place
   if (threadIdx.x <= 1)
-    for (int j = 0; j < ns; ++j) y[j] = plant_x[(size_t)b * ns + j];
+    for (int j = 0; j < ns; ++j) y[j] = plant_x[(size_t)p * ns + j];
   __syncthreads();
   if (threadIdx.x > 1) return;
   const bool simulate = threadIdx.x == 0;
@@ -1446,7 +1448,7 @@ __device__ void omg_cl_tail(int b, int ode, int ns, int ni, int n_samp, double d
     for (int i = 0; i < ts * ni; ++i) A[i] = disturb ? U[i] + D[i] : U[i];
     if (lag) {                                      // u' = (u_cmd - u) / tau from the applied input
       double ua[OMG_CL_MAX_INPUT];
-      for (int c = 0; c < ni; ++c) ua[c] = plant_u[(size_t)b * ni + c];
+      for (int c = 0; c < ni; ++c) ua[c] = plant_u[(size_t)p * ni + c];
       for (int i = 0; i < n_samp; ++i) {
         for (int c = 0; c < ni; ++c) {
           const double c0 = A[i * ni + c], c1 = A[(i + 1) * ni + c], cm = 0.5 * (c0 + c1), u = ua[c];
@@ -1475,15 +1477,18 @@ __device__ void omg_cl_tail(int b, int ode, int ns, int ni, int n_samp, double d
   }
   double* xo = simulate ? plant_x_next : pred_x;
   double* uo = simulate ? plant_u_next : pred_u;
-  for (int j = 0; j < ns; ++j) xo[(size_t)b * ns + j] = y[j];
-  for (int c = 0; c < ni; ++c) uo[(size_t)b * ni + c] = Uin[n_samp * ni + c];
+  for (int j = 0; j < ns; ++j) xo[(size_t)p * ns + j] = y[j];
+  for (int c = 0; c < ni; ++c) uo[(size_t)p * ni + c] = Uin[n_samp * ni + c];
 }
 
-// One block per instance; both halves start from the plant state x_p(t_k) and the trajectory
-// just solved, sampled at t_k + s*dt, s = 0..n_samp (omg_cl_tail).  R = [nd][n_samp+1][L]: row d
-// is the d-th derivative of the basis divided by T^d, nd the rows the model reads.  `model`
-// selects the planned-input map, `ode` the right-hand side (omg_ode_models).
-__global__ void omg_closed_loop_kernel(int model, int ode, int nd, int ns, int ni, int n, const double* __restrict__ x,
+// One block per (instance b, vehicle v), block p = b*n_veh + v; both halves start from the plant
+// state x_p(t_k) and the trajectory just solved, sampled at t_k + s*dt, s = 0..n_samp (omg_cl_tail).
+// Vehicle v's input splines are the ni columns of length L at x[b, veh_off[v]...].  R =
+// [nd][n_samp+1][L]: row d is the d-th derivative of the basis divided by T^d, nd the rows the
+// model reads.  `model` selects the planned-input map, `ode` the right-hand side (omg_ode_models).
+// A single vehicle is n_veh = 1 at offset 0.
+__global__ void omg_closed_loop_kernel(int model, int ode, int nd, int ns, int ni, int n, int n_veh,
+                                       const int* __restrict__ veh_off, const double* __restrict__ x,
                                        int L, int n_samp, const double* __restrict__ R,
                                        double dt, int lag, double tau, int disturb, int n_traj,
                                        const double* __restrict__ filt, const double* __restrict__ mean,
@@ -1493,11 +1498,11 @@ __global__ void omg_closed_loop_kernel(int model, int ode, int nd, int ns, int n
                                        double* __restrict__ pred_x, double* __restrict__ pred_u,
                                        double* __restrict__ scratch) {
   OMG_DYN_SHARED(sm);
-  const int b = blockIdx.x, ts = n_samp + 1;
+  const int p = blockIdx.x, b = p / n_veh, v = p - b * n_veh, ts = n_samp + 1;
   double* U = sm;                // planned input [ts][ni]
   double* D = sm + ts * ni;      // filtered disturbance [ts][ni]
   double* A = sm + 2 * ts * ni;  // input reaching the ODE [ts][ni]
-  const double* xb = x + (size_t)b * n;
+  const double* xb = x + (size_t)b * n + veh_off[v];
   const size_t nr = (size_t)ts * L;
   for (int s = threadIdx.x; s < ts; s += blockDim.x) {
     double v[4][OMG_CL_MAX_INPUT];
@@ -1505,8 +1510,9 @@ __global__ void omg_closed_loop_kernel(int model, int ode, int nd, int ns, int n
       for (int c = 0; c < ni; ++c) v[d][c] = omg_row_dot(R + d * nr + (size_t)s * L, xb + c * L, L);
     omg_cl_input_map(model, ni, v, U + s * ni);
   }
-  omg_cl_tail(b, ode, ns, ni, n_samp, dt, lag, tau, disturb, n_traj, filt, mean, stdev, seed, step, plant_x,
-              plant_u, plant_x_next, plant_u_next, pred_x, pred_u, scratch, (size_t)n_traj + 2 * OMG_CL_PAD, U, D, A);
+  omg_cl_tail(b, p, v * ni, ode, ns, ni, n_samp, dt, lag, tau, disturb, n_traj, filt, mean, stdev, seed, step,
+              plant_x, plant_u, plant_x_next, plant_u_next, pred_x, pred_u, scratch, (size_t)n_traj + 2 * OMG_CL_PAD,
+              U, D, A);
 }
 
 // trajectory sampling: out[b, blk, c, s] = sum_k S_blk[s,k] * x[b, off_blk + c*len_blk + k]
@@ -1797,7 +1803,7 @@ __global__ void omg_closed_loop_free_kernel(int model, int ode, int nd, int ns, 
     omg_cl_input_map(model, ni, v, U + s * ni);
   }
   const int ntr = n_traj ? n_traj[b] : 0;
-  omg_cl_tail(b, ode, ns, ni, nsb, dt, lag, tau, disturb && ntr > 0, ntr, filt, mean, stdev, seed, step, plant_x,
+  omg_cl_tail(b, b, 0, ode, ns, ni, nsb, dt, lag, tau, disturb && ntr > 0, ntr, filt, mean, stdev, seed, step, plant_x,
               plant_u, plant_x_next, plant_u_next, pred_x, pred_u, scratch, stride, U, D, A);
 }
 
@@ -2884,11 +2890,13 @@ int omg_integrate_rk4(int32_t model, int32_t B, int32_t n_state, int32_t n_input
   return 0;
 }
 
-// omg_closed_loop_step and omg_closed_loop_step_der; `fn` names the caller in the messages.  R
-// holds the rows [n_der][n_samp+1][L], except row 1 when R1 is given (omg_closed_loop_step's
-// separate R0 and R1).
-static int closed_loop_launch(const char* fn, int32_t model, int32_t B, int32_t n_state, int32_t n_input, int32_t n,
-                              const double* x, int32_t L, int32_t n_samp, int32_t n_der, const double* R,
+// omg_closed_loop_step, omg_closed_loop_step_der and omg_closed_loop_step_fleet; `fn` names the
+// caller in the messages.  R holds the rows [n_der][n_samp+1][L], except row 1 when R1 is given
+// (omg_closed_loop_step's separate R0 and R1).  veh_off [n_veh]: host offsets of the vehicles'
+// spline blocks in x.
+static int closed_loop_launch(const char* fn, int32_t model, int32_t B, int32_t n_veh, int32_t n_state,
+                              int32_t n_input, int32_t n, const double* x, const int32_t* veh_off, int32_t L,
+                              int32_t n_samp, int32_t n_der, const double* R,
                               const double* R1, double sample_time, int32_t lag, double time_constant, int32_t disturb, int32_t n_traj,
                               const double* filt, const double* mean, const double* stdev, uint64_t seed,
                               int32_t step, const double* plant_x, const double* plant_u, double* plant_x_next,
@@ -2897,6 +2905,13 @@ static int closed_loop_launch(const char* fn, int32_t model, int32_t B, int32_t 
   if (model < 0 || model >= OMG_ODE_N_MODELS) { set_err(f + ": unknown vehicle model " + std::to_string(model)); return -1; }
   const bool sizes_ok = omg_ode_sizes_ok(model, n_state, n_input) && n_input <= OMG_CL_MAX_INPUT && n >= n_input * L;
   if (!sizes_ok || L < 1 || n_samp < 0) { set_err(f + ": bad state / input / spline sizes"); return -1; }
+  if (n_veh < 1) { set_err(f + ": n_veh must be >= 1, got " + std::to_string(n_veh)); return -1; }
+  if (!veh_off) { set_err(f + ": null argument (vehicle offsets)"); return -1; }
+  for (int v = 0; v < n_veh; ++v)
+    if (veh_off[v] < 0 || (int64_t)veh_off[v] + (int64_t)n_input * L > n) {
+      set_err(f + ": vehicle " + std::to_string(v) + " at offset " + std::to_string(veh_off[v]) + ": its " +
+              std::to_string(n_input) + " input splines of length " + std::to_string(L) + " leave x of " +
+              std::to_string(n) + " variables"); return -1; }
   if (n_der < omg_ode_models[model].n_der || n_der > 4) {
     set_err(f + ": vehicle model " + std::to_string(model) + " needs " + std::to_string(omg_ode_models[model].n_der) +
             " to 4 derivative rows, got " + std::to_string(n_der)); return -1; }
@@ -2911,6 +2926,7 @@ static int closed_loop_launch(const char* fn, int32_t model, int32_t B, int32_t 
   if (!x || !R || !plant_x || !plant_u || !plant_x_next || !plant_u_next || !pred_x || !pred_u ||
       (disturb && (!filt || !mean || !stdev || !scratch))) { set_err(f + ": null argument"); return -1; }
   if (B <= 0) return 0;
+  if ((int64_t)B * n_veh > 0x7fffffff) { set_err(f + ": B * n_veh exceeds 2^31 - 1 blocks"); return -1; }
   cudaStream_t stream = (cudaStream_t)stream_;
   // host descriptors -> device: R (the rows the model reads) | filt (11) | mean | stdev
   const size_t nr = (size_t)(n_samp + 1) * L, nR = (size_t)omg_ode_models[model].n_der * nr;
@@ -2927,11 +2943,11 @@ static int closed_loop_launch(const char* fn, int32_t model, int32_t B, int32_t 
   int device = 0;
   CK(cudaGetDevice(&device));
   static thread_local DescCache cache;
-  if (desc_upload(cache, device, std::vector<int>(1, 0), dv.data(), dv.size(), stream)) return -1;
+  if (desc_upload(cache, device, std::vector<int>(veh_off, veh_off + n_veh), dv.data(), dv.size(), stream)) return -1;
   const double* d = cache.d_d;
   const size_t smem = sizeof(double) * 3 * (size_t)(n_samp + 1) * n_input;
-  OMG_LAUNCH(omg_closed_loop_kernel, B, 32, smem, stream, model, omg_ode_models[model].ode,
-             omg_ode_models[model].n_der, n_state, n_input, n, x,
+  OMG_LAUNCH(omg_closed_loop_kernel, B * n_veh, 32, smem, stream, model, omg_ode_models[model].ode,
+             omg_ode_models[model].n_der, n_state, n_input, n, n_veh, cache.d_i, x,
              L, n_samp, d, sample_time, lag, time_constant, disturb, n_traj, d + nR, d + nR + 11,
              d + nR + 11 + n_input, seed, step, plant_x, plant_u, plant_x_next, plant_u_next, pred_x, pred_u, scratch);
   CK(cudaGetLastError());
@@ -2944,9 +2960,22 @@ int omg_closed_loop_step_der(int32_t model, int32_t B, int32_t n_state, int32_t 
                              const double* mean, const double* stdev, uint64_t seed, int32_t step,
                              const double* plant_x, const double* plant_u, double* plant_x_next,
                              double* plant_u_next, double* pred_x, double* pred_u, double* scratch, void* stream) {
-  return closed_loop_launch("omg_closed_loop_step_der", model, B, n_state, n_input, n, x, L, n_samp, n_der, R,
-                            nullptr, sample_time, lag, time_constant, disturb, n_traj, filt, mean, stdev, seed, step, plant_x,
-                            plant_u, plant_x_next, plant_u_next, pred_x, pred_u, scratch, stream);
+  const int32_t off0 = 0;
+  return closed_loop_launch("omg_closed_loop_step_der", model, B, 1, n_state, n_input, n, x, &off0, L, n_samp, n_der,
+                            R, nullptr, sample_time, lag, time_constant, disturb, n_traj, filt, mean, stdev, seed, step,
+                            plant_x, plant_u, plant_x_next, plant_u_next, pred_x, pred_u, scratch, stream);
+}
+
+int omg_closed_loop_step_fleet(int32_t model, int32_t B, int32_t n_veh, int32_t n_state, int32_t n_input, int32_t n,
+                               const double* x, const int32_t* veh_off, int32_t L, int32_t n_samp, int32_t n_der,
+                               const double* R, double sample_time, int32_t lag, double time_constant,
+                               int32_t disturb, int32_t n_traj, const double* filt, const double* mean,
+                               const double* stdev, uint64_t seed, int32_t step, const double* plant_x,
+                               const double* plant_u, double* plant_x_next, double* plant_u_next, double* pred_x,
+                               double* pred_u, double* scratch, void* stream) {
+  return closed_loop_launch("omg_closed_loop_step_fleet", model, B, n_veh, n_state, n_input, n, x, veh_off, L, n_samp,
+                            n_der, R, nullptr, sample_time, lag, time_constant, disturb, n_traj, filt, mean, stdev,
+                            seed, step, plant_x, plant_u, plant_x_next, plant_u_next, pred_x, pred_u, scratch, stream);
 }
 
 int omg_closed_loop_step(int32_t model, int32_t B, int32_t n_state, int32_t n_input, int32_t n, const double* x,
@@ -2958,7 +2987,8 @@ int omg_closed_loop_step(int32_t model, int32_t B, int32_t n_state, int32_t n_in
   if (model != OMG_ODE_INTEGRATOR && model != OMG_ODE_QUADROTOR3D) {
     set_err("omg_closed_loop_step: unknown vehicle model " + std::to_string(model)); return -1; }
   if (!R1) R0 = nullptr;                            // (reported as a null argument)
-  return closed_loop_launch("omg_closed_loop_step", model, B, n_state, n_input, n, x, L, n_samp, 2, R0, R1,
+  const int32_t off0 = 0;
+  return closed_loop_launch("omg_closed_loop_step", model, B, 1, n_state, n_input, n, x, &off0, L, n_samp, 2, R0, R1,
                             sample_time, lag, time_constant, disturb, n_traj, filt, mean, stdev, seed, step, plant_x,
                             plant_u, plant_x_next, plant_u_next, pred_x, pred_u, scratch, stream);
 }

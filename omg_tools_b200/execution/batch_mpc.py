@@ -1,6 +1,6 @@
 """Batched receding-horizon driver: B independent copies of one Point2point
 scenario (Holonomic, Holonomic3D, Quadrotor3D, Dubins, HolonomicOrient, planar Quadrotor or
-SimpleQuadrotor3D vehicle) advance in lock step,
+SimpleQuadrotor3D vehicle, or a fleet of Holonomic / Holonomic3D vehicles) advance in lock step,
 every MPC step is ONE batched solve on the GPU.
 
 It is the batched counterpart of the reference's ``Simulator.run()`` /
@@ -25,7 +25,15 @@ first-order actuator lag (simulate: the next plant state), once on the clean pla
 (predict: state0 of the next solve).  Options read from the vehicle: ideal_update,
 ideal_prediction, 1storder_delay, time_constant, input_disturbance {fc, stdev, mean}; the noise
 is keyed by ``seed``, the MPC step and the instance, so a realisation does not depend on the
-batch size.  history['plant'] and history['plant_input'] hold the plant state and the last
+batch size.
+
+Several vehicles in one problem (inter-vehicle avoidance, the central formation) run with a fixed horizon for fleets
+of Holonomic or Holonomic3D vehicles that share one spline basis and one set of plant options: one adapter per
+vehicle (``vehs``; ``veh`` is vehicle 0) reads its splines at its own column of x, the jitter shifts all starts of an
+instance by one vector and all goals by another, the closed loop is ONE launch for the fleet
+(omg_closed_loop_step_fleet; vehicle v's noise is signal v * n_input + j of the instance), and ``state``, ``inp``,
+``poseT`` and history['state'|'plant'|'plant_input'] are [B, n_veh, ·].  Any other multi-vehicle problem raises
+NotImplementedError naming the cause.  history['plant'] and history['plant_input'] hold the plant state and the last
 applied input at every update boundary.  ``sample_time`` is the simulation grid of the plant
 and of the obstacle motion (the reference simulator's sample_time, 0.01 s by default).
 
@@ -53,8 +61,9 @@ class _HolonomicAdapter(object):
 
     N_DER = 2       # rows of spline derivatives the plant step reads (value, first derivative)
 
-    def __init__(self, mpc, vehicle, batch, jitter, rng):
+    def __init__(self, mpc, vehicle, batch, jitter, rng, x_off=0):
         self.mpc, self.v = mpc, vehicle
+        self.x_off = x_off      # column of the vehicle's splines in x (several vehicles in one problem)
         self.nd = nd = vehicle.n_dim
         rep = lambda a: np.repeat(np.asarray(a, float)[None], batch, 0)
         self.state, self.inp = rep(vehicle.prediction['state']), rep(vehicle.prediction['input'])
@@ -64,9 +73,9 @@ class _HolonomicAdapter(object):
             self.poseT[1:] += rng.uniform(-jitter, jitter, (batch - 1, nd))
 
     def cold_start(self, X0):
-        L = len(self.v.basis)
+        L, o = len(self.v.basis), self.x_off
         for k in range(self.nd):
-            X0[:, k * L:(k + 1) * L] = np.linspace(self.state[:, k], self.poseT[:, k], L).T
+            X0[:, o + k * L:o + (k + 1) * L] = np.linspace(self.state[:, k], self.poseT[:, k], L).T
 
     def pack(self, P, off):
         v, nd = self.v.label, self.nd
@@ -83,14 +92,14 @@ class _HolonomicAdapter(object):
         B1 = Bd.eval_basis([tau]).dot(P1) / T
         L = len(basis)
         if device:
-            out = sample_batch(X, [(0, L, nd, np.vstack([B0, B1]))]).cpu().numpy()
+            out = sample_batch(X, [(self.x_off, L, nd, np.vstack([B0, B1]))]).cpu().numpy()
             # layout: [column][sample] with samples (value, derivative)
             for k in range(nd):
                 self.state[:, k], self.inp[:, k] = out[:, 2 * k], out[:, 2 * k + 1]
         else:
             Xh = X.cpu().numpy()
             for k in range(nd):
-                c = Xh[:, k * L:(k + 1) * L]
+                c = Xh[:, self.x_off + k * L:self.x_off + (k + 1) * L]
                 self.state[:, k] = c.dot(B0[0])
                 self.inp[:, k] = c.dot(B1[0])
 
@@ -477,6 +486,42 @@ def _adapter_for(vehicle):
     return _ADAPTERS[name]
 
 
+# the vehicle classes BatchMPC runs several of in one problem, and the options they must share
+_FLEET = ('Holonomic', 'Holonomic3D')
+_FLEET_OPTIONS = ('ideal_update', 'ideal_prediction', '1storder_delay', 'time_constant', 'input_disturbance')
+
+
+def _check_fleet(problem, free_T):
+    """Raise NotImplementedError, naming the cause, for a multi-vehicle problem BatchMPC does not run:
+    a free motion time (the Trailer's problem among them), a vehicle that is not simulated, a mixed fleet, a class other than
+    Holonomic / Holonomic3D, differing spline bases or differing plant options."""
+    vehicles = problem.vehicles
+    if free_T:
+        raise NotImplementedError('BatchMPC runs a free end time (FreeTPoint2point) for one vehicle only, '
+                                  'this problem has %d' % len(vehicles))
+    for v in vehicles:
+        if not getattr(v, 'to_simulate', True):
+            raise NotImplementedError('BatchMPC cannot run %s with several vehicles: it has to_simulate = False'
+                                      % type(v).__name__)
+    names = sorted(set(type(v).__name__ for v in vehicles))
+    if len(names) > 1:
+        raise NotImplementedError('BatchMPC runs fleets of one vehicle class only, not a mixed fleet of %s'
+                                  % ', '.join(names))
+    if names[0] not in _FLEET:
+        raise NotImplementedError('BatchMPC runs several vehicles of class Holonomic or Holonomic3D only, not %s'
+                                  % names[0])
+    b0 = vehicles[0].basis
+    for v in vehicles[1:]:
+        if v.basis.degree != b0.degree or not np.array_equal(np.asarray(v.basis.knots), np.asarray(b0.knots)):
+            raise NotImplementedError('BatchMPC runs fleets with one spline basis only: %s and %s differ in '
+                                      'degree or knots' % (vehicles[0].label, v.label))
+        for key in _FLEET_OPTIONS:
+            a, b = vehicles[0].options.get(key), v.options.get(key)
+            if repr(a) != repr(b):
+                raise NotImplementedError('BatchMPC runs fleets with equal plant options only: option %r of %s '
+                                          'and %s differ' % (key, vehicles[0].label, v.label))
+
+
 class BatchMPC(object):
 
     def __init__(self, problem, batch, update_time=0.1, jitter=0.0, seed=0, device_predict=True,
@@ -484,6 +529,10 @@ class BatchMPC(object):
         import torch
         from ..problems.point2point import FreeTPoint2point
         self.free_T = isinstance(problem, FreeTPoint2point)
+        self.vehicles = problem.vehicles
+        self.fleet = len(self.vehicles) > 1
+        if self.fleet:
+            _check_fleet(problem, self.free_T)
         if self.free_T:
             vehicle, opt = problem.vehicles[0], problem.vehicles[0].options
             if type(vehicle).__name__ not in _FREE_T:
@@ -512,8 +561,21 @@ class BatchMPC(object):
         self.dev = dev
         rng = np.random.default_rng(seed)
         n, m = self.tb.n, self.tb.m
-        # per-instance scenario data (host); the vehicle-specific part lives in the adapter
-        self.veh = _adapter_for(self.vehicle)(self, self.vehicle, batch, jitter, rng)
+        # per-instance scenario data (host); the vehicle-specific part lives in the adapters, one per
+        # vehicle, each reading its vehicle's splines at their own column of x
+        if self.fleet:
+            var = self.father._var_struct.entries
+            self.vehs = [_adapter_for(v)(self, v, batch, 0., rng, x_off=var[(v.label, 'splines_seg0')][0])
+                         for v in self.vehicles]
+            if jitter > 0:      # one shift of all starts and one of all goals: the fleet keeps its geometry
+                nd = self.vehs[0].nd
+                d0, dT = rng.uniform(-jitter, jitter, (batch - 1, nd)), rng.uniform(-jitter, jitter, (batch - 1, nd))
+                for a in self.vehs:
+                    a.state[1:] += d0
+                    a.poseT[1:] += dT
+        else:
+            self.vehs = [_adapter_for(self.vehicle)(self, self.vehicle, batch, jitter, rng)]
+        self.veh = self.vehs[0]
         self.obs = []
         for o in self.obstacles:
             d = {'x': np.repeat(o.signals['position'][:, -1][None], batch, 0).astype(float),
@@ -529,7 +591,8 @@ class BatchMPC(object):
         self.off = {key: ent[key][0] for key in ent}
         # cold start per instance (holonomic.py:118-127, quadrotor3d.py:189-201)
         X0 = np.repeat(self.father.get_variables().cat[None], batch, 0)
-        self.veh.cold_start(X0)
+        for a in self.vehs:
+            a.cold_start(X0)
         self.X = torch.tensor(X0, device=dev)
         self.Xn = torch.empty_like(self.X)
         self.LAM = torch.empty((batch, m), dtype=torch.float64, device=dev)
@@ -574,7 +637,7 @@ class BatchMPC(object):
         sample_time = self.sample_time
         self.seed, self.k = seed, 0
         self.model = ODE_MODELS[type(self.vehicle).__name__]
-        self.plant_x = torch.tensor(self.state, device=self.dev)
+        self.plant_x = torch.tensor(self.state, device=self.dev)      # ([B, n_veh, n] for a fleet)
         self.plant_u = torch.tensor(self.inp, device=self.dev)
         self.pred_x, self.pred_u = torch.empty_like(self.plant_x), torch.empty_like(self.plant_u)
         lag = opt.get('1storder_delay', False) and not self.ideal_update
@@ -582,25 +645,33 @@ class BatchMPC(object):
         self.disturbance = None
         dist = opt.get('input_disturbance')
         if dist and not self.ideal_update:
-            ni = self.plant_u.shape[1]
+            ni = self.plant_u.shape[-1]
             stdev = np.broadcast_to(np.asarray(dist['stdev'], dtype=float), (ni,))
             mean = np.broadcast_to(np.asarray(dist.get('mean', np.zeros(ni)), dtype=float), (ni,))
             # (a free motion time grows the scratch with the longest trajectory of a step)
             n_traj = int(np.round(self.T / sample_time, 6)) + 1 if self.T is not None else 0
-            scratch = torch.empty(self.B * ni * (n_traj + 24), dtype=torch.float64, device=self.dev)
+            scratch = torch.empty(self.B * len(self.vehs) * ni * (n_traj + 24), dtype=torch.float64,
+                                  device=self.dev)
             self.disturbance = (disturbance_filter(dist['fc']), mean, stdev, scratch)
         self.history['plant'] = [self.plant_x.cpu().numpy().copy()]
         self.history['plant_input'] = [self.plant_u.cpu().numpy().copy()]
 
-    # state / input / target of every instance (owned by the vehicle adapter)
-    state = property(lambda self: self.veh.state)
-    inp = property(lambda self: self.veh.inp)
-    poseT = property(lambda self: self.veh.poseT)
+    # state / input / target of every instance (owned by the vehicle adapters): [B, n] for one
+    # vehicle, [B, n_veh, n] for a fleet
+    def _stacked(self, key):
+        if self.fleet:
+            return np.stack([getattr(a, key) for a in self.vehs], axis=1)
+        return getattr(self.veh, key)
+
+    state = property(lambda self: self._stacked('state'))
+    inp = property(lambda self: self._stacked('inp'))
+    poseT = property(lambda self: self._stacked('poseT'))
 
     # ------------------------------------------------------------------
     def _pack_parameters(self, t):
         P, off = self.P, self.off
-        self.veh.pack(P, off)
+        for a in self.vehs:
+            a.pack(P, off)
         for o, d in zip(self.obstacles, self.obs):
             nd = o.n_dim
             for key in ('x', 'v', 'a'):
@@ -656,7 +727,8 @@ class BatchMPC(object):
         if self.closed_loop:
             self._plant_step(t_rel)
         else:
-            self.veh.predict(self.X, t_rel, self.update_time, self.T, device=self.device_predict)
+            for a in self.vehs:
+                a.predict(self.X, t_rel, self.update_time, self.T, device=self.device_predict)
         self._advance_obstacles(self.update_time, self.sample_time)
         self.history['state'].append(self.state.copy())
         self.time = np.round(t + self.update_time, 6)
@@ -664,10 +736,12 @@ class BatchMPC(object):
     def _plant_step(self, t_rel):
         """Reference Vehicle.simulate and predict (vehicle.py:302-337, 359-392) of every instance
         in one launch; the ideal half of a mixed setting follows the spline as before."""
-        from ..solver.b200 import closed_loop_step
+        from ..solver.b200 import closed_loop_step, closed_loop_step_fleet
         n_samp = int(np.round(self.update_time / self.sample_time, 6))
         higher = None
-        if self.veh.N_DER > 2:
+        if self.fleet:
+            R = plant_rows_der(self.vehicle.basis, self.T, t_rel, self.sample_time, n_samp)[:self.veh.N_DER]
+        elif self.veh.N_DER > 2:
             R = plant_rows_der(self.vehicle.basis, self.T, t_rel, self.sample_time, n_samp)
             R0, R1, higher = R[0], R[1], R[2:self.veh.N_DER]
         else:
@@ -677,13 +751,19 @@ class BatchMPC(object):
             filt, mean, stdev, scratch = self.disturbance
             n_traj = int(np.round((self.T - t_rel) / self.sample_time, 6)) + 1
             dist = (filt, mean, stdev, n_traj, scratch)
-        closed_loop_step(self.model, self.X, len(self.vehicle.basis), R0, R1, self.sample_time,
-                         self.plant_x, self.plant_u,
-                         (self.plant_x, self.plant_u, self.pred_x, self.pred_u), self.k, seed=self.seed,
-                         time_constant=self.time_constant, disturbance=dist, higher=higher)
+        out = (self.plant_x, self.plant_u, self.pred_x, self.pred_u)
+        if self.fleet:          # one launch for every (instance, vehicle)
+            closed_loop_step_fleet(self.model, self.X, [a.x_off for a in self.vehs], len(self.vehicle.basis), R,
+                                   self.sample_time, self.plant_x, self.plant_u, out, self.k, seed=self.seed,
+                                   time_constant=self.time_constant, disturbance=dist)
+        else:
+            closed_loop_step(self.model, self.X, len(self.vehicle.basis), R0, R1, self.sample_time,
+                             self.plant_x, self.plant_u, out, self.k, seed=self.seed,
+                             time_constant=self.time_constant, disturbance=dist, higher=higher)
         self.k += 1
         if self.ideal_prediction or self.ideal_update:
-            self.veh.predict(self.X, t_rel, self.update_time, self.T, device=self.device_predict)
+            for a in self.vehs:
+                a.predict(self.X, t_rel, self.update_time, self.T, device=self.device_predict)
         elif hasattr(self.veh, 'predict_planned'):
             # signals other than state and input come from the planned trajectory (vehicle.py:326-328)
             self.veh.predict_planned(self.X, t_rel, self.update_time, self.T, device=self.device_predict)
@@ -693,8 +773,12 @@ class BatchMPC(object):
         if not self.ideal_prediction:
             # (copies: the adapter updates its arrays in place, and on a CPU device .numpy()
             # would share the kernel's output buffers)
-            self.veh.state = self.pred_x.cpu().numpy().copy()
-            self.veh.inp = self.pred_u.cpu().numpy().copy()
+            px, pu = self.pred_x.cpu().numpy(), self.pred_u.cpu().numpy()
+            if self.fleet:
+                for v, a in enumerate(self.vehs):
+                    a.state, a.inp = px[:, v].copy(), pu[:, v].copy()
+            else:
+                self.veh.state, self.veh.inp = px.copy(), pu.copy()
         self.history['plant'].append(self.plant_x.cpu().numpy().copy())
         self.history['plant_input'].append(self.plant_u.cpu().numpy().copy())
 

@@ -524,21 +524,28 @@ def config_free_end(options=None, build_solver=True):
     return problem
 
 
-def config_interveh(options=None, build_solver=True):
+def config_interveh(options=None, build_solver=True, start_offset=0.):
     """examples/p2p_holonomic_interveh_avoidance.py: two Holonomic vehicles swapping places
     across an empty Square(5) room, one NLP, separating hyperplanes between the vehicles
-    (Environment.define_intervehicle_collision_constraints)."""
+    (Environment.define_intervehicle_collision_constraints).  start_offset moves vehicle 0's
+    start off the head-on line (config_interveh_offset)."""
     N = 2
     vehicles = [Holonomic() for _ in range(N)]
     for k, vehicle in enumerate(vehicles):
         vehicle.set_initial_conditions([1.5 * np.cos((k * 2. * np.pi) / N),
-                                        1.5 * np.sin((k * 2. * np.pi) / N)])
+                                        1.5 * np.sin((k * 2. * np.pi) / N) + (start_offset if k == 0 else 0.)])
         vehicle.set_terminal_conditions([-1.5 * np.cos((k * 2. * np.pi) / N),
                                          -1.5 * np.sin((k * 2. * np.pi) / N)])
     environment = Environment(room={'shape': Square(5.)})
     opts = {'inter_vehicle_avoidance': True}
     opts.update(options or {})
     return _p2p(vehicles, environment, opts, build_solver)
+
+
+def config_interveh_offset(options=None, build_solver=True):
+    """config_interveh with vehicle 0 starting 0.1 m off the head-on line: with the symmetric
+    start, rounding decides on which side the vehicles pass each other."""
+    return config_interveh(options, build_solver, start_offset=0.1)
 
 
 def config_formation_central_example(options=None, build_solver=True):

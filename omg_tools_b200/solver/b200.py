@@ -87,7 +87,7 @@ EXPORTS = ['omg_abi_version', 'omg_last_error', 'omg_default_options',
            'omg_tables_free', 'omg_integrate_rk4', 'omg_feas_batch', 'omg_feas_batch_host',
            'omg_comm_unique_id', 'omg_comm_create', 'omg_comm_destroy', 'omg_admm_exchange_x',
            'omg_admm_zl_update_dist', 'omg_closed_loop_step', 'omg_closed_loop_step_der',
-           'omg_shift_free_batch', 'omg_eval_batch', 'omg_closed_loop_step_free']
+           'omg_shift_free_batch', 'omg_eval_batch', 'omg_closed_loop_step_free', 'omg_closed_loop_step_fleet']
 
 _lib = None
 
@@ -147,6 +147,9 @@ def bind(lib):
     lib.omg_closed_loop_step_der.argtypes = ([C.c_int32] * 5 + [vp, C.c_int32, C.c_int32, C.c_int32, vp,
                                              C.c_double, C.c_int32, C.c_double, C.c_int32, C.c_int32,
                                              vp, vp, vp, C.c_uint64, C.c_int32] + [vp] * 8)
+    lib.omg_closed_loop_step_fleet.argtypes = ([C.c_int32] * 6 + [vp, vp, C.c_int32, C.c_int32, C.c_int32, vp,
+                                               C.c_double, C.c_int32, C.c_double, C.c_int32, C.c_int32,
+                                               vp, vp, vp, C.c_uint64, C.c_int32] + [vp] * 8)
     lib.omg_closed_loop_step_free.argtypes = ([C.c_int32] * 5 + [vp] + [C.c_int32] * 4 + [vp, C.c_int32, C.c_int32,
                                               vp, vp, C.c_double, C.c_int32, C.c_double, C.c_int32,
                                               vp, vp, vp, C.c_uint64, C.c_int32] + [vp] * 8)
@@ -820,6 +823,54 @@ def closed_loop_step(model, X, L, R0, R1, sample_time, plant_x, plant_u, out, st
         R = np.ascontiguousarray(np.concatenate(rows))
         rc = lib.omg_closed_loop_step_der(mid, B, ns, ni, X.shape[1], X.data_ptr(), L, R0.shape[0] - 1,
                                           R.shape[0], R.ctypes.data, *rest)
+    if rc != 0:
+        raise RuntimeError('libomgb200: %s' % lib.omg_last_error().decode())
+
+
+def closed_loop_step_fleet(model, X, offsets, L, R, sample_time, plant_x, plant_u, out, step, seed=0,
+                           time_constant=None, disturbance=None, stream=None):
+    """closed_loop_step for a fleet of vehicles of one model and one spline basis in every row of X
+    (omg_closed_loop_step_fleet): vehicle v's input splines start at column offsets[v] of X.
+    R: the derivative rows [n_der, n_samp + 1, L] (plant_rows_der; n_der from the model's to 4).
+    plant_x [B, n_veh, n_state], plant_u [B, n_veh, n_input] and the four tensors of ``out`` carry
+    a vehicle axis; disturbance = (filt, mean, stdev, n_traj, scratch) with scratch of at least
+    B * n_veh * n_input * (n_traj + 24) elements.  The noise of vehicle v's input j is keyed as
+    signal v * n_input + j of the instance.  Every other argument is closed_loop_step's."""
+    lib = load_library()
+    mid = ODE_MODELS[model] if isinstance(model, str) else int(model)
+    tensors = (X, plant_x, plant_u) + tuple(out)
+    if plant_x.dim() != 3 or plant_u.dim() != 3:
+        raise ValueError('plant_x / plant_u must be [B, n_veh, n_state | n_input]')
+    B, nv, ns = plant_x.shape
+    ni = plant_u.shape[2]
+    offsets = np.ascontiguousarray(offsets, dtype=np.int32).reshape(-1)
+    if offsets.size != nv or tuple(plant_u.shape[:2]) != (B, nv):
+        raise ValueError('one spline offset per vehicle of plant_x / plant_u')
+    d = disturbance is not None
+    if d:
+        filt, mean, stdev, n_traj, scratch = disturbance
+        tensors += (scratch,)
+        if scratch.numel() < B * nv * ni * (n_traj + 24):
+            raise ValueError('disturbance scratch too small')
+        filt, mean, stdev = (np.ascontiguousarray(a, dtype=np.float64) for a in (filt, mean, stdev))
+        if filt.size != 11 or mean.size != ni or stdev.size != ni:
+            raise ValueError('disturbance filter / mean / stdev sizes')
+    on_gpu = _check_device_tensors(tensors, lib)
+    if X.dim() != 2 or X.shape[0] != B:
+        raise ValueError('X must be [B, n] with the batch of plant_x')
+    for t, shape in zip(out, ((B, nv, ns), (B, nv, ni), (B, nv, ns), (B, nv, ni))):
+        if tuple(t.shape) != shape:
+            raise ValueError('output tensor shapes do not match the plant state / input')
+    R = np.ascontiguousarray(R, dtype=np.float64)
+    if R.ndim != 3 or R.shape[2] != L:
+        raise ValueError('R must be [n_der, n_samp + 1, L]')
+    rc = lib.omg_closed_loop_step_fleet(
+        mid, B, nv, ns, ni, X.shape[1], X.data_ptr(), offsets.ctypes.data, int(L), R.shape[1] - 1, R.shape[0],
+        R.ctypes.data, float(sample_time), int(time_constant is not None),
+        float(time_constant) if time_constant is not None else 0., int(d), int(n_traj) if d else 0,
+        filt.ctypes.data if d else None, mean.ctypes.data if d else None, stdev.ctypes.data if d else None,
+        int(seed) & 0xFFFFFFFFFFFFFFFF, int(step), plant_x.data_ptr(), plant_u.data_ptr(),
+        *[t.data_ptr() for t in out], scratch.data_ptr() if d else None, _stream_handle(on_gpu, X.device, stream))
     if rc != 0:
         raise RuntimeError('libomgb200: %s' % lib.omg_last_error().decode())
 
