@@ -230,6 +230,14 @@ int omg_get_info(omg_problem* h, int32_t* n, int32_t* m, int32_t* n_par,
  * "sparse LDL^T: N=200 nnz(L)=3861 levels=29 root=36 pairs=41088 nt=128 ctas/SM=4 smem=53104"
  * or "envelope kernels (intermediates)").  Valid until the handle is destroyed. */
 const char* omg_structure_info(omg_problem* h);
+/* Layout of the envelope kernels for this problem (the kernels of inertia_mode = 1 and of what
+ * the sparse kernel does not take): "kernel=<standard|xl> nt=<threads per block>
+ * K=<shared|scratch> V=<shared|scratch> arrays-in-scratch=<per-instance arrays in scratch>
+ * max-panel-rows=.. min-panel-rows=.. N%8=.. wide=<0|1>" -- where the KKT envelope K and the
+ * parameter tape V live, the most and fewest rows a panel of the factorisation reaches (the
+ * last panel, which reaches only the right-hand side, left out of the fewest), and whether
+ * panels reach more rows than a block has threads.  Valid until the handle is destroyed. */
+const char* omg_envelope_layout(omg_problem* h);
 /* Device time (ms) and kernel-launch count of the last omg_solve_batch,
  * measured with CUDA events on the caller's stream. */
 int omg_last_timing(omg_problem* h, float* kernel_ms, int32_t* launches);

@@ -234,6 +234,10 @@ OMG_DYN_SHARED(sm);
 // Pivot j must satisfy sign[j]*pivot > PIV_TOL*|K_jj| (variables) or > 0
 // (equality rows); otherwise ctl->fail (eq_fail for an equality pivot).
 // ---------------------------------------------------------------------------
+// WIDE: a panel may reach more rows than the block has threads (max_panel_rows + 2 > NT); the
+// rows from NT on then go to a loop strided by NT.  A separate instantiation, so the kernels of
+// every other problem keep the code (and registers) of one row per thread.
+template <bool WIDE>
 __device__ __forceinline__ void factor_env(const DevTab& T, const Smem& S, double* K, Ctl* ctl, double* pc,
                                            const int mode) {
   const int tid = threadIdx.x;
@@ -312,8 +316,9 @@ __device__ __forceinline__ void factor_env(const DevTab& T, const Smem& S, doubl
     // ---- 2. panel solve over the rows this panel reaches ----------------------
     const int p0 = pptr[pb];
     const int nrows = pptr[pb + 1] - p0;
-    if (tid < nrows) {
-      const int rr = tid;
+    double2* P2 = reinterpret_cast<double2*>(Pt);
+    double2* PS2 = reinterpret_cast<double2*>(PtS);
+    auto solve_row = [&](const int rr) {
       const int r = prow[p0 + rr];
       const int rb = eptr[r] - efirst[r];
       rbase[rr] = rb; rrow[rr] = r;
@@ -334,19 +339,24 @@ __device__ __forceinline__ void factor_env(const DevTab& T, const Smem& S, doubl
       for (int c = 0; c < NB; ++c) if (c < nb) Kr[c] = a[c];
       // panel buffers as double2 [column pair][row]: conflict-free stores here, and
       // at most 2-way conflicts for the 2x2-tile loads of the trailing update
-      double2* P2 = reinterpret_cast<double2*>(Pt);
-      double2* PS2 = reinterpret_cast<double2*>(PtS);
 #pragma unroll
       for (int q = 0; q < NB / 2; ++q) {
         const double v0 = (2 * q < nb) ? a[2 * q] : 0.0, v1 = (2 * q + 1 < nb) ? a[2 * q + 1] : 0.0;
         P2[q * LDP + rr] = make_double2(v0, v1);
         PS2[q * LDP + rr] = make_double2(sg[2 * q] * v0, sg[2 * q + 1] * v1);
       }
-    } else if (tid < nrows + 2 && tid < LDP) {   // zero padding rows for the 2x2 tiles
-      double2* P2 = reinterpret_cast<double2*>(Pt);
-      double2* PS2 = reinterpret_cast<double2*>(PtS);
+    };
+    auto zero_row = [&](const int rr) {   // zero padding rows nrows, nrows + 1 for the 2x2 tiles
 #pragma unroll
-      for (int q = 0; q < NB / 2; ++q) { P2[q * LDP + tid] = make_double2(0.0, 0.0); PS2[q * LDP + tid] = make_double2(0.0, 0.0); }
+      for (int q = 0; q < NB / 2; ++q) { P2[q * LDP + rr] = make_double2(0.0, 0.0); PS2[q * LDP + rr] = make_double2(0.0, 0.0); }
+    };
+    if (tid < nrows) solve_row(tid);
+    else if (tid < nrows + 2 && tid < LDP) zero_row(tid);
+    if constexpr (WIDE) {   // row rr on thread rr % NT
+      for (int rr = tid + NT; rr < nrows + 2 && rr < LDP; rr += NT) {
+        if (rr < nrows) solve_row(rr);
+        else zero_row(rr);
+      }
     }
     __syncthreads();
     FT(8);
@@ -481,7 +491,7 @@ __device__ __forceinline__ void jac_xl(const DevTab& T, const double* __restrict
 // ---------------------------------------------------------------------------
 // XL = true: problems with intermediates (n_mid > 0) and/or a KKT envelope / parameter tape
 // that exceeds shared memory: V (and K if needed) live in the block's L2-resident scratch.
-template <bool XL>
+template <bool XL, bool WIDE>
 __device__ __forceinline__ void ipm_body(const DevTab& T, const omg_options& O, const Batch& A, const Smem& S) {
   __shared__ Ctl ctl;
   __shared__ double phase_cyc[NPHASE];
@@ -914,7 +924,7 @@ __device__ __forceinline__ void ipm_body(const DevTab& T, const omg_options& O, 
         }
         }
         TICK(6);   // W + border + rhs
-        factor_env(T, S, K, &ctl, tracing ? phase_cyc : nullptr, O.inertia_mode);
+        factor_env<WIDE>(T, S, K, &ctl, tracing ? phase_cyc : nullptr, O.inertia_mode);
         __syncthreads();
         phase_t0 = clock64();
         if (!ctl.fail) break;
@@ -1202,8 +1212,8 @@ __device__ __forceinline__ void ipm_body(const DevTab& T, const omg_options& O, 
   }
 }
 
-__global__ void __launch_bounds__(512, 1)
-omg_ipm_kernel(const DevTab T, const omg_options O, const Batch A, const Smem S) { ipm_body<false>(T, O, A, S); }
+template <bool WIDE> __global__ void __launch_bounds__(512, 1)
+omg_ipm_kernel(const DevTab T, const omg_options O, const Batch A, const Smem S) { ipm_body<false, WIDE>(T, O, A, S); }
 
 // sparse variant (omg_sp.cuh): L D L^T on the minimum-degree structure, thread streams, 128 or
 // 256 threads per instance, as many blocks per SM as shared memory allows (config 2: 3)
@@ -1215,16 +1225,16 @@ omg_ipm_kernel_sp(const __grid_constant__ DevTab T, const __grid_constant__ SpTa
   ipm_body_sp(T, P, O, A, S);
 }
 
-__global__ void __launch_bounds__(256, 2)
-omg_ipm_kernel_2cta(const DevTab T, const omg_options O, const Batch A, const Smem S) { ipm_body<false>(T, O, A, S); }
+template <bool WIDE> __global__ void __launch_bounds__(256, 2)
+omg_ipm_kernel_2cta(const DevTab T, const omg_options O, const Batch A, const Smem S) { ipm_body<false, WIDE>(T, O, A, S); }
 
-__global__ void __launch_bounds__(512, 1)
-omg_ipm_kernel_xl(const DevTab T, const omg_options O, const Batch A, const Smem S) { ipm_body<true>(T, O, A, S); }
+template <bool WIDE> __global__ void __launch_bounds__(512, 1)
+omg_ipm_kernel_xl(const DevTab T, const omg_options O, const Batch A, const Smem S) { ipm_body<true, WIDE>(T, O, A, S); }
 
 // XL with K in scratch: the block needs little shared memory, and the kernel is bound by the
 // latency of its L2 streams, so two blocks per SM overlap better than one wide block
-__global__ void __launch_bounds__(256, 2)
-omg_ipm_kernel_xl_2cta(const DevTab T, const omg_options O, const Batch A, const Smem S) { ipm_body<true>(T, O, A, S); }
+template <bool WIDE> __global__ void __launch_bounds__(256, 2)
+omg_ipm_kernel_xl_2cta(const DevTab T, const omg_options O, const Batch A, const Smem S) { ipm_body<true, WIDE>(T, O, A, S); }
 
 // warm-start shift: x[b, off + c*len + i] <- sum_k T[i,k] x[b, off + c*len + k]
 __global__ void omg_shift_kernel(double* x, int B, int n, int n_blocks, const int* offs,
@@ -2107,6 +2117,8 @@ struct omg_problem {
   // launch configuration of the envelope kernels (kept: inertia_mode = 1 is tied to the
   // envelope's elimination order and always runs there)
   int env_nt = 0, env_ctas = 0; size_t env_smem_bytes = 0;
+  bool wide = false;   // factor_env's strided panel solve (WIDE instantiation of the envelope kernels)
+  std::string env_info;   // omg_envelope_layout
 };
 
 template <typename Tp>
@@ -2445,9 +2457,9 @@ omg_problem* omg_problem_create(const omg_tables* tb, const omg_options* opt, in
   {
     cudaFuncAttributes f0, fx;
     size_t b0 = 0, bx = 0;
-    if (cudaFuncGetAttributes(&f0, (const void*)omg_ipm_kernel) == cudaSuccess)
+    if (cudaFuncGetAttributes(&f0, (const void*)omg_ipm_kernel<false>) == cudaSuccess)
       b0 = (size_t)prop.sharedMemPerBlockOptin - f0.sharedSizeBytes;
-    if (cudaFuncGetAttributes(&fx, (const void*)omg_ipm_kernel_xl) == cudaSuccess)
+    if (cudaFuncGetAttributes(&fx, (const void*)omg_ipm_kernel_xl<false>) == cudaSuccess)
       bx = (size_t)prop.sharedMemPerBlockOptin - fx.sharedSizeBytes;
     h->xl = (n_mid > 0) || layout(true, true) > b0;
     if (h->xl) {
@@ -2461,7 +2473,7 @@ omg_problem* omg_problem_create(const omg_tables* tb, const omg_options* opt, in
   // blocks per SM: 2 x 256 threads overlap one block's serial pivots with the other's
   // parallel phases; 1 x 512 keeps every per-instance array in shared memory.
   cudaFuncAttributes fa;
-  if (ok && cudaFuncGetAttributes(&fa, h->xl ? (const void*)omg_ipm_kernel_xl : (const void*)omg_ipm_kernel) != cudaSuccess) { set_err("cudaFuncGetAttributes failed"); ok = false; }
+  if (ok && cudaFuncGetAttributes(&fa, h->xl ? (const void*)omg_ipm_kernel_xl<false> : (const void*)omg_ipm_kernel<false>) != cudaSuccess) { set_err("cudaFuncGetAttributes failed"); ok = false; }
   const size_t budget1 = ok ? (size_t)prop.sharedMemPerBlockOptin - fa.sharedSizeBytes : 0;
   const size_t budget2 = ok ? ((size_t)prop.sharedMemPerMultiprocessor - 2 * 1024) / 2 - fa.sharedSizeBytes : 0;
   {
@@ -2470,8 +2482,11 @@ omg_problem* omg_problem_create(const omg_tables* tb, const omg_options* opt, in
     h->target_ctas = (want == 2 && (!h->xl || !k_in_smem) && (size_t)off * 8 <= budget2) ? 2 : 1;
     h->nt = (h->target_ctas == 1) ? 512 : 256;
   }
-  const void* kfn = h->xl ? ((h->target_ctas == 1) ? (const void*)omg_ipm_kernel_xl : (const void*)omg_ipm_kernel_xl_2cta)
-                          : (h->target_ctas == 1) ? (const void*)omg_ipm_kernel : (const void*)omg_ipm_kernel_2cta;
+  h->wide = T.max_panel_rows + 2 > h->nt;   // panels reach more rows than the block has threads
+  const void* kfn = h->wide ? (h->xl ? ((h->target_ctas == 1) ? (const void*)omg_ipm_kernel_xl<true> : (const void*)omg_ipm_kernel_xl_2cta<true>)
+                                     : (h->target_ctas == 1) ? (const void*)omg_ipm_kernel<true> : (const void*)omg_ipm_kernel_2cta<true>)
+                            : (h->xl ? ((h->target_ctas == 1) ? (const void*)omg_ipm_kernel_xl<false> : (const void*)omg_ipm_kernel_xl_2cta<false>)
+                                     : (h->target_ctas == 1) ? (const void*)omg_ipm_kernel<false> : (const void*)omg_ipm_kernel_2cta<false>);
   const size_t budget = (h->target_ctas == 1) ? budget1 : budget2;
   if (ok && (size_t)off * 8 > budget) {
     char buf[256];
@@ -2512,6 +2527,21 @@ omg_problem* omg_problem_create(const omg_tables* tb, const omg_options* opt, in
       const char* e = getenv("OMG_B200_KERNEL");   // "envelope": force the envelope kernels
       std::string why;
       h->env_nt = h->nt; h->env_ctas = h->ctas_per_sm; h->env_smem_bytes = h->smem_bytes;
+      {  // the envelope kernels' layout (they run inertia_mode = 1 and what the sparse kernel
+         // rejects); min-panel-rows leaves out the last panel, which reaches only the
+         // right-hand-side row
+        int arr_scratch = 0;
+        for (int k = 0; k < N_ARR; ++k) arr_scratch += (S.arr[k] < 0) ? 1 : 0;
+        int min_rows = tb->kkt_panel_ptr[1] - tb->kkt_panel_ptr[0];
+        for (int pb = 1; pb + 1 < T.n_panels; ++pb)
+          min_rows = std::min(min_rows, tb->kkt_panel_ptr[pb + 1] - tb->kkt_panel_ptr[pb]);
+        h->env_info = std::string("kernel=") + (h->xl ? "xl" : "standard") + " nt=" + std::to_string(h->env_nt) +
+                      " K=" + (S.K >= 0 ? "shared" : "scratch") + " V=" + (S.V >= 0 ? "shared" : "scratch") +
+                      " arrays-in-scratch=" + std::to_string(arr_scratch) +
+                      " max-panel-rows=" + std::to_string(T.max_panel_rows) +
+                      " min-panel-rows=" + std::to_string(min_rows) + " N%8=" + std::to_string(N % NB) +
+                      " wide=" + (h->wide ? "1" : "0");
+      }
       if (!(e && strcmp(e, "envelope") == 0) && sp_setup(h, tb, prop, &why)) {
         h->sp = true;
         h->nt = h->P.nt; h->ctas_per_sm = h->sp_ctas;
@@ -2571,6 +2601,7 @@ int omg_get_info(omg_problem* h, int32_t* n, int32_t* m, int32_t* n_par, int32_t
 }
 
 const char* omg_structure_info(omg_problem* h) { return h ? h->sp_info.c_str() : ""; }
+const char* omg_envelope_layout(omg_problem* h) { return h ? h->env_info.c_str() : ""; }
 
 int omg_solve_batch(omg_problem* h, int32_t B, const double* x0, const double* p,
                     const double* lbg, const double* ubg, int32_t bounds_shared,
@@ -2602,10 +2633,16 @@ int omg_solve_batch(omg_problem* h, int32_t B, const double* x0, const double* p
   CK(cudaMemsetAsync(h->counter, 0, sizeof(int), stream));
   CK(cudaEventRecord(h->ev0, stream));
   if (use_sp) OMG_LAUNCH(omg_ipm_kernel_sp, grid, h->P.nt, h->sp_smem_bytes, stream, h->T, h->P, h->opt, A, h->SS);
-  else if (h->xl && h->target_ctas == 1) OMG_LAUNCH(omg_ipm_kernel_xl, grid, 512, h->env_smem_bytes, stream, h->T, h->opt, A, h->S);
-  else if (h->xl) OMG_LAUNCH(omg_ipm_kernel_xl_2cta, grid, 256, h->env_smem_bytes, stream, h->T, h->opt, A, h->S);
-  else if (h->target_ctas == 1) OMG_LAUNCH(omg_ipm_kernel, grid, 512, h->env_smem_bytes, stream, h->T, h->opt, A, h->S);
-  else OMG_LAUNCH(omg_ipm_kernel_2cta, grid, 256, h->env_smem_bytes, stream, h->T, h->opt, A, h->S);
+  else if (h->wide) {
+    if (h->xl && h->target_ctas == 1) OMG_LAUNCH(omg_ipm_kernel_xl<true>, grid, 512, h->env_smem_bytes, stream, h->T, h->opt, A, h->S);
+    else if (h->xl) OMG_LAUNCH(omg_ipm_kernel_xl_2cta<true>, grid, 256, h->env_smem_bytes, stream, h->T, h->opt, A, h->S);
+    else if (h->target_ctas == 1) OMG_LAUNCH(omg_ipm_kernel<true>, grid, 512, h->env_smem_bytes, stream, h->T, h->opt, A, h->S);
+    else OMG_LAUNCH(omg_ipm_kernel_2cta<true>, grid, 256, h->env_smem_bytes, stream, h->T, h->opt, A, h->S);
+  }
+  else if (h->xl && h->target_ctas == 1) OMG_LAUNCH(omg_ipm_kernel_xl<false>, grid, 512, h->env_smem_bytes, stream, h->T, h->opt, A, h->S);
+  else if (h->xl) OMG_LAUNCH(omg_ipm_kernel_xl_2cta<false>, grid, 256, h->env_smem_bytes, stream, h->T, h->opt, A, h->S);
+  else if (h->target_ctas == 1) OMG_LAUNCH(omg_ipm_kernel<false>, grid, 512, h->env_smem_bytes, stream, h->T, h->opt, A, h->S);
+  else OMG_LAUNCH(omg_ipm_kernel_2cta<false>, grid, 256, h->env_smem_bytes, stream, h->T, h->opt, A, h->S);
   CK(cudaGetLastError());
   CK(cudaEventRecord(h->ev1, stream));
   h->timed = true; h->launches = 1;

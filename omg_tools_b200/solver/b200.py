@@ -82,7 +82,7 @@ class _Options(C.Structure):
 EXPORTS = ['omg_abi_version', 'omg_last_error', 'omg_default_options',
            'omg_problem_create', 'omg_problem_destroy', 'omg_set_options',
            'omg_solve_batch', 'omg_solve_batch_host', 'omg_shift_batch',
-           'omg_get_trace', 'omg_get_info', 'omg_structure_info', 'omg_last_timing',
+           'omg_get_trace', 'omg_get_info', 'omg_structure_info', 'omg_envelope_layout', 'omg_last_timing',
            'omg_admm_zl_update', 'omg_sample_batch', 'omg_tables_read',
            'omg_tables_free', 'omg_integrate_rk4', 'omg_feas_batch', 'omg_feas_batch_host',
            'omg_comm_unique_id', 'omg_comm_create', 'omg_comm_destroy', 'omg_admm_exchange_x',
@@ -130,6 +130,8 @@ def bind(lib):
     lib.omg_get_info.argtypes = [vp] + [_i32p] * 6
     lib.omg_structure_info.argtypes = [vp]
     lib.omg_structure_info.restype = C.c_char_p
+    lib.omg_envelope_layout.argtypes = [vp]
+    lib.omg_envelope_layout.restype = C.c_char_p
     lib.omg_comm_unique_id.argtypes = [vp]
     lib.omg_comm_create.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32]
     lib.omg_comm_create.restype = C.c_void_p
@@ -416,6 +418,12 @@ class B200Solver(object):
     def structure(self):
         """One-line report of the kernel family / factor structure chosen for this problem."""
         return self.lib.omg_structure_info(self._handle).decode()
+
+    @property
+    def envelope_layout(self):
+        """Layout of the envelope kernels for this problem (include/omg_b200.h,
+        omg_envelope_layout)."""
+        return self.lib.omg_envelope_layout(self._handle).decode()
 
     def last_timing(self):
         ms, nl = C.c_float(), C.c_int32()
