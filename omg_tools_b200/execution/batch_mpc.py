@@ -37,11 +37,14 @@ NotImplementedError naming the cause.  history['plant'] and history['plant_input
 applied input at every update boundary.  ``sample_time`` is the simulation grid of the plant
 and of the obstacle motion (the reference simulator's sample_time, 0.01 s by default).
 
-With a FreeTPoint2point (T a decision variable; Holonomic, Holonomic3D and Dubins) every instance
+With a FreeTPoint2point (T a decision variable; Holonomic, Holonomic3D, Dubins, HolonomicOrient, the planar
+Quadrotor and SimpleQuadrotor3D) every instance
 runs the reference's free-T loop on its own motion time (point2point.py:300-374): the warm start
 re-expresses the splines with shift_spline from the instance's T [omg_shift_free_batch], only the
 instances still running are solved, the prediction samples each plan at its own
-tau = min(dt, T) / T [omg_eval_batch], and an instance stops for good when T < dt or at its goal.
+tau = min(dt, T) / T [omg_eval_batch], and an instance stops for good when T < dt or at its goal (the
+adapter's ``arrived``: the quadrotors compare their position with the target and test the planned
+velocity dspl, which the closed loop also reads from the plan at each instance's own tau).
 history['T'] and history['active'] hold the motion times and the instances solved at every step.
 The free-T loop runs ideal, or closed with ideal_prediction off (ideal_update on or off): one launch
 [omg_closed_loop_step_free] on the whole batch samples each moving instance's plan on its own time
@@ -108,6 +111,10 @@ class _HolonomicAdapter(object):
         own tau1 = min(dt, T) / T, value and first derivative / T (omg_eval_batch)."""
         out = _eval(X, blocks, tau1[:, None], T, 2).reshape(-1, self.nd, 2)   # [b][column][derivative]
         self.state[idx], self.inp[idx] = out[:, :, 0], out[:, :, 1]
+
+    def arrived(self, state, inp, idx, tol):
+        """Free-T stop test of the instances idx (holonomic.py check_terminal_conditions)."""
+        return _at_goal(state, inp, self.poseT[idx], tol)
 
     def position(self):
         return self.state
@@ -230,6 +237,12 @@ def _put(P, off, label, name, val):
     P[:, off[(label, name)]:off[(label, name)] + val.shape[1]] = val
 
 
+def _at_goal(state, inp, poseT, tol):
+    """check_terminal_conditions of the vehicles whose state is their pose: the state at the target
+    and the input at rest (the reference's (a > tol or b) > tol, for stop_tol < 1)."""
+    return (np.linalg.norm(state - poseT, axis=1) <= tol) & (np.linalg.norm(inp, axis=1) <= tol)
+
+
 class _DubinsAdapter(object):
     """Dubins (dubins.py, every formulation): the decision splines are v~ and tg = tan(theta/2);
     the position is the running integral of v~ (1 - tg^2), 2 v~ tg re-anchored at the previous
@@ -303,6 +316,10 @@ class _DubinsAdapter(object):
                                 st[:, 1] + T * np.einsum('bq,bq->b', vt * (2 * tg), wts), 2 * np.arctan2(tg1, 1)]
         self.inp[idx] = np.c_[vt1 * q1, 2 * dtg1 / q1]
 
+    def arrived(self, state, inp, idx, tol):
+        """Free-T stop test of the instances idx (dubins.py check_terminal_conditions)."""
+        return _at_goal(state, inp, self.poseT[idx], tol)
+
     def position(self):
         return self.state[:, :2]
 
@@ -338,13 +355,28 @@ class _HolonomicOrientAdapter(object):
         _put(P, off, v, 'posT', self.poseT[:, :2])
         _put(P, off, v, 'tg_haT', np.tan(self.poseT[:, 2] / 2))
 
+    @staticmethod
+    def _maps(out):
+        """State and input from the values and first derivatives of x, y and tg, out [B, 6] laid out
+        column / derivative (splines2signals)."""
+        tg, dtg = out[:, 4], out[:, 5]
+        return (np.c_[out[:, 0], out[:, 2], 2 * np.arctan2(tg, 1)],
+                np.c_[out[:, 1], out[:, 3], 2 * dtg / (1 + tg**2)])
+
     def predict(self, X, t_rel, dt, T, device=True):
         basis = self.v.basis
         R = _rows(basis, [(t_rel + dt) / T], T, 2)
         out = _sample(X, len(basis), 3, np.vstack([R[0], R[1]]), device)   # column: value, derivative
-        tg, dtg = out[:, 4], out[:, 5]
-        self.state = np.c_[out[:, 0], out[:, 2], 2 * np.arctan2(tg, 1)]
-        self.inp = np.c_[out[:, 1], out[:, 3], 2 * dtg / (1 + tg**2)]
+        self.state, self.inp = self._maps(out)
+
+    def predict_free(self, X, idx, tau1, T, blocks):
+        """Free motion time: state and input of the instances idx (X holds their rows) at their own
+        tau1 = min(dt, T) / T (omg_eval_batch)."""
+        self.state[idx], self.inp[idx] = self._maps(_eval(X, blocks, tau1[:, None], T, 2))
+
+    def arrived(self, state, inp, idx, tol):
+        """Free-T stop test of the instances idx (holonomicorient.py check_terminal_conditions)."""
+        return _at_goal(state, inp, self.poseT[idx], tol)
 
     def position(self):
         return self.state[:, :2]
@@ -387,19 +419,39 @@ class _QuadrotorAdapter(object):
         out = _sample(X, len(basis), 2, _rows(basis, [tau1], T, 4)[:, 0], device)
         return out.reshape(-1, 2, 4)
 
-    def predict(self, X, t_rel, dt, T, device=True):
-        s, g = self._signals(X, (t_rel + dt) / T, T, device), self.v.g
+    def _maps(self, s):
+        """State, input, dspl and ddspl from x, y and their derivatives 1..3, s [B, 2, 4]."""
+        g = self.v.g
         (x, dx, ddx, dddx), (y, dy, ddy, dddy) = s[:, 0].T, s[:, 1].T
-        self.state = np.c_[x, y, dx, dy, np.arctan2(ddx, ddy + g)]
-        self.inp = np.c_[np.sqrt(ddx**2 + (ddy + g)**2),
-                         (dddx * (ddy + g) - ddx * dddy) / ((ddy + g)**2 + ddx**2)]
-        self.dspl, self.ddspl = s[:, :, 1].copy(), s[:, :, 2].copy()
+        return (np.c_[x, y, dx, dy, np.arctan2(ddx, ddy + g)],
+                np.c_[np.sqrt(ddx**2 + (ddy + g)**2), (dddx * (ddy + g) - ddx * dddy) / ((ddy + g)**2 + ddx**2)],
+                s[:, :, 1].copy(), s[:, :, 2].copy())
+
+    def predict(self, X, t_rel, dt, T, device=True):
+        self.state, self.inp, self.dspl, self.ddspl = self._maps(self._signals(X, (t_rel + dt) / T, T, device))
 
     def predict_planned(self, X, t_rel, dt, T, device=True):
         """The signals that the non-ideal prediction still takes from the planned trajectory
         (reference vehicle.py:326-328): dspl and ddspl at t + dt."""
         s = self._signals(X, (t_rel + dt) / T, T, device)
         self.dspl, self.ddspl = s[:, :, 1].copy(), s[:, :, 2].copy()
+
+    def predict_free(self, X, idx, tau1, T, blocks):
+        """Free motion time: state, input, dspl and ddspl of the instances idx (X holds their rows) at
+        their own tau1 = min(dt, T) / T, derivatives 0..3 in one omg_eval_batch launch."""
+        s = _eval(X, blocks, tau1[:, None], T, 4).reshape(-1, 2, 4)          # [b][column][derivative]
+        self.state[idx], self.inp[idx], self.dspl[idx], self.ddspl[idx] = self._maps(s)
+
+    def predict_planned_free(self, X, idx, tau1, T, blocks):
+        """predict_planned with a free motion time: dspl and ddspl of the instances idx at their own tau1."""
+        s = _eval(X, blocks, tau1[:, None], T, 3).reshape(-1, 2, 3)
+        self.dspl[idx], self.ddspl[idx] = s[:, :, 1], s[:, :, 2]
+
+    def arrived(self, state, inp, idx, tol):
+        """Free-T stop test of the instances idx (quadrotor.py check_terminal_conditions): the position
+        part of the state at the target and the planned velocity dspl at rest; the input is not read."""
+        return ((np.linalg.norm(state[:, :2] - self.poseT[idx], axis=1) <= tol) &
+                (np.linalg.norm(self.dspl[idx], axis=1) <= tol))
 
     def position(self):
         return self.state[:, :2]
@@ -420,6 +472,7 @@ class _SimpleQuadrotor3DAdapter(object):
         if jitter > 0:
             self.state[1:, :3] += rng.uniform(-jitter, jitter, (batch - 1, 3))
             self.poseT[1:, :3] += rng.uniform(-jitter, jitter, (batch - 1, 3))
+        self.vel_plan = self.state[:, 3:6].copy()     # the planned velocity (signals['dspl']) of the free-T stop test
 
     def cold_start(self, X0):
         L = len(self.v.basis)
@@ -436,8 +489,13 @@ class _SimpleQuadrotor3DAdapter(object):
         _put(P, off, v, 'positionT', self.poseT)
 
     def predict(self, X, t_rel, dt, T, device=True):
-        basis, g = self.v.basis, self.v.g
+        basis = self.v.basis
         s = _sample(X, len(basis), 3, _rows(basis, [(t_rel + dt) / T], T, 4)[:, 0], device).reshape(-1, 3, 4)
+        self.state, self.inp = self._maps(s)
+
+    def _maps(self, s):
+        """State and input from x, y, z and their derivatives 1..3, s [B, 3, 4]."""
+        g = self.v.g
         pos, vel = s[:, :, 0], s[:, :, 1]
         (ddx, ddy, ddz), (dddx, dddy, dddz) = s[:, :, 2].T, s[:, :, 3].T
         az = ddz + g
@@ -447,8 +505,25 @@ class _SimpleQuadrotor3DAdapter(object):
         u2 = (-dddy * (ddx**2 + az**2) + ddy * (ddx * dddx + dddz * az)) / \
             ((ddx**2 + ddy**2 + az**2) * np.sqrt(ddx**2 + az**2))
         u3 = (az * dddx - ddx * dddz) / (az**2 + ddx**2)
-        self.state = np.c_[pos, vel, phi, theta]
-        self.inp = np.c_[u1, u2, u3]
+        return np.c_[pos, vel, phi, theta], np.c_[u1, u2, u3]
+
+    def predict_free(self, X, idx, tau1, T, blocks):
+        """Free motion time: state, input and planned velocity of the instances idx (X holds their
+        rows) at their own tau1 = min(dt, T) / T, derivatives 0..3 in one omg_eval_batch launch."""
+        s = _eval(X, blocks, tau1[:, None], T, 4).reshape(-1, 3, 4)          # [b][column][derivative]
+        self.state[idx], self.inp[idx] = self._maps(s)
+        self.vel_plan[idx] = s[:, :, 1]
+
+    def predict_planned_free(self, X, idx, tau1, T, blocks):
+        """The planned velocity (signals['dspl'], which the closed loop takes from the plan,
+        vehicle.py:371-374) of the instances idx at their own tau1."""
+        self.vel_plan[idx] = _eval(X, blocks, tau1[:, None], T, 2).reshape(-1, 3, 2)[:, :, 1]
+
+    def arrived(self, state, inp, idx, tol):
+        """Free-T stop test of the instances idx (quadrotor3d_simple.py check_terminal_conditions): the
+        position part of the state at the target and the planned velocity (signals['dspl']) at rest."""
+        return ((np.linalg.norm(state[:, :3] - self.poseT[idx], axis=1) <= tol) &
+                (np.linalg.norm(self.vel_plan[idx], axis=1) <= tol))
 
     def position(self):
         return self.state[:, :3]
@@ -471,7 +546,7 @@ def plant_rows_der(basis, T, t_rel, sample_time, n_samp):
 
 
 # the adapters with a per-instance prediction for a free motion time (predict_free)
-_FREE_T = ('Holonomic', 'Holonomic3D', 'Dubins')
+_FREE_T = ('Holonomic', 'Holonomic3D', 'Dubins', 'HolonomicOrient', 'Quadrotor', 'SimpleQuadrotor3D')
 
 _ADAPTERS = {'Holonomic': _HolonomicAdapter, 'Holonomic3D': _HolonomicAdapter,
              'Quadrotor3D': _Quadrotor3DAdapter, 'Dubins': _DubinsAdapter,
@@ -823,10 +898,15 @@ class BatchMPC(object):
         move = T >= self.sample_time
         if self.closed_loop:
             self._plant_step_free(act, move, T)
-        if move.any() and (not self.closed_loop or self.ideal_update):
+        if move.any():
             sel = torch.from_numpy(np.nonzero(move)[0]).to(self.dev)
-            self.veh.predict_free(Xn.index_select(0, sel) if not move.all() else Xn, act[move],
-                                  np.minimum(dt, T[move]) / T[move], T[move], self.veh_blocks)
+            args = (Xn.index_select(0, sel) if not move.all() else Xn, act[move],
+                    np.minimum(dt, T[move]) / T[move], T[move], self.veh_blocks)
+            if not self.closed_loop or self.ideal_update:
+                self.veh.predict_free(*args)
+            elif hasattr(self.veh, 'predict_planned_free'):
+                # signals other than state and input come from the plan (vehicle.py:326-328, 371-374)
+                self.veh.predict_planned_free(*args)
         if self.closed_loop:
             moved = act[move]
             if self.ideal_update and len(moved):
@@ -840,15 +920,13 @@ class BatchMPC(object):
             self.history['plant'].append(px)
             self.history['plant_input'].append(pu)
             # the reference's check_terminal_conditions reads the plant (signals)
-            pos, inp = px[act], pu[act]
+            state, inp = px[act], pu[act]
         else:
-            pos, inp = self.state[act], self.inp[act]
+            state, inp = self.state[act], self.inp[act]
         self._advance_obstacles(dt, self.sample_time)
         self.history['state'].append(self.state.copy())
         self.time = np.round(self.time + dt, 6)
-        tol = self.vehicle.options['stop_tol']
-        arrived = ((np.linalg.norm(pos - self.poseT[act], axis=1) <= tol) &
-                   (np.linalg.norm(inp, axis=1) <= tol))
+        arrived = self.veh.arrived(state, inp, act, self.vehicle.options['stop_tol'])
         self.active[act[(T < dt) | arrived]] = False
 
     def _plant_step_free(self, act, move, T):

@@ -342,6 +342,54 @@ def config_dubins_freeT(options=None, build_solver=True, init_v_til=0.):
     return _p2p(vehicle, environment, options, build_solver, freeT=True)
 
 
+def config_holonomic_orient_freeT(options=None, build_solver=True):
+    """examples/p2p_holonomic_orient.py as written: the scene of config_holonomic_orient with a free
+    end time (n=151, m=2961, n_par=55)."""
+    from . import HolonomicOrient, Rectangle
+    vehicle = HolonomicOrient()
+    vehicle.set_options({'reg_type': 'norm_1', 'reg_weight': 10})
+    vehicle.set_initial_conditions([-1.5, -1.5, np.pi / 4.])
+    vehicle.set_terminal_conditions([2., 2., np.pi / 2.])
+    environment = Environment(room={'shape': Square(5.)})
+    rectangle = Rectangle(width=3., height=0.2)
+    environment.add_obstacle(Obstacle({'position': [-1.8, -0.5]}, shape=rectangle))
+    environment.add_obstacle(Obstacle({'position': [1.7, -0.5]}, shape=rectangle))
+    trajectories = {'velocity': {'time': [3., 4.], 'values': [[-0.15, 0.0], [0., 0.15]]}}
+    environment.add_obstacle(Obstacle({'position': [1.5, 0.5]}, shape=Circle(0.4),
+                                      simulation={'trajectories': trajectories}))
+    return _p2p(vehicle, environment, options, build_solver, freeT=True)
+
+
+def config_quadrotor2d_freeT(options=None, build_solver=True):
+    """The scene of config_quadrotor2d (examples/p2p_quadrotor.py) with a free end time
+    (n=76, m=443, n_par=27)."""
+    from . import Quadrotor
+    vehicle = Quadrotor()
+    vehicle.set_options({'safety_distance': 0.1})
+    vehicle.set_initial_conditions([-4., -4., 0., 0., 0.])
+    vehicle.set_terminal_conditions([4., 4.])
+    environment = Environment(room={'shape': Square(10.)})
+    environment.add_obstacle(Obstacle({'position': [-0.6, -5.4]},
+                                      shape=Rectangle(width=0.2, height=12.)))
+    return _p2p(vehicle, environment, options, build_solver, freeT=True)
+
+
+def config_quadrotor3d_simple_freeT(options=None, build_solver=True):
+    """The scene of config_quadrotor3d_simple with a free end time (n=159, m=833, n_par=63)."""
+    from . import SimpleQuadrotor3D, Cuboid, Plate, Rectangle
+    vehicle = SimpleQuadrotor3D(0.5)
+    vehicle.set_initial_conditions([-3, -2, -0.5, 0, 0, 0, 0, 0])
+    vehicle.set_terminal_conditions([3, 2, 0.5])
+    vehicle.set_options({'safety_distance': 0.1, 'safety_weight': 10})
+    environment = Environment(room={'shape': Cuboid(8, 6, 8)})
+    plate = lambda: Plate(Rectangle(5., 8.), 0.1, orientation=[0., np.pi / 2, 0.])
+    trajectory = {'velocity': {'time': [1.5], 'values': [[0, 0, -0.6]]}}
+    environment.add_obstacle(Obstacle({'position': [-2, 0, -2]}, shape=plate()))
+    environment.add_obstacle(Obstacle({'position': [2, 0, 3.5]}, shape=plate(),
+                                      simulation={'trajectories': trajectory}))
+    return _p2p(vehicle, environment, options, build_solver, freeT=True)
+
+
 def config_trailer(options=None, build_solver=True, init_v_til=0.):
     """examples/p2p_trailer.py: a Dubins vehicle (Circle(0.2), 9 knot intervals) pulling a
     Rectangle(0.2, 0.2) trailer on a 0.6 m hitch from (0, 0, 0) to (3.4, 3, 0), trailer heading

@@ -1,9 +1,12 @@
 """Cost of the batched MPC loop with a free motion time (execution/batch_mpc.py, FreeTPoint2point).
 
-    python tools/freet_mpc_bench.py [--steps 40] [--closed] [--out DIR]
+    python tools/freet_mpc_bench.py [--steps 40] [--closed] [--scenario NAME [--batch 256]] [--out DIR]
 
 Two workloads at 0.5 s updates: config_freeT with a jittered batch of 1024 (jitter 0.1) and
-config_dubins_freeT (init_v_til = 0.3) with a jittered batch of 256.  Each runs until every
+config_dubins_freeT (init_v_til = 0.3) with a jittered batch of 256; --scenario (repeatable) runs
+the named scenarios of omg_tools_b200/scenarios.py instead, each with a jittered batch of --batch
+(e.g. config_holonomic_orient_freeT, config_quadrotor2d_freeT, config_quadrotor3d_simple_freeT).
+Each runs until every
 instance stopped or --steps updates.  Reported per workload and step: the wall time of the MPC
 step (closed by a device synchronise), the solve time (CUDA events around the solve launch), the
 time of the warm-start (omg_shift_free_batch) and prediction (omg_eval_batch) launches alone (CUDA
@@ -12,7 +15,7 @@ the warm start, shift_spline on every shifted block of each active instance (wha
 loop does per instance), is timed on the instances and motion times of the second step.  With
 --closed the loops run through the vehicle's own dynamics at the reference's vehicle defaults
 (ideal_update and ideal_prediction off) with the first-order lag (time constant 0.1) and the input
-disturbance (fc 0.01, stdev 0.05), and the plant step (omg_closed_loop_step_free) is timed like the
+disturbance (fc 0.01, stdev 0.05 on every input), and the plant step (omg_closed_loop_step_free) is timed like the
 other launches; the host's shift_spline is not timed then.  The card's
 name and power limit are read in the same call.  Needs a CUDA device; prints one JSON line and
 writes it to DIR/freet_mpc_bench.json when --out is given."""
@@ -31,7 +34,7 @@ sys.path.insert(0, ROOT)
 WORKLOADS = [('config_freeT', 1024, {}), ('config_dubins_freeT', 256, {'init_v_til': 0.3})]
 DT = 0.5
 CLOSED = {'ideal_update': False, 'ideal_prediction': False, '1storder_delay': True, 'time_constant': 0.1,
-          'input_disturbance': {'fc': 0.01, 'stdev': 0.05 * np.ones(2)}}
+          'input_disturbance': {'fc': 0.01, 'stdev': 0.05}}
 
 
 def card():
@@ -117,19 +120,23 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--steps', type=int, default=40)
     ap.add_argument('--closed', action='store_true', help='closed loop with lag and disturbance')
+    ap.add_argument('--scenario', action='append', default=None, help='scenario name (repeatable)')
+    ap.add_argument('--batch', type=int, default=256, help='batch of the --scenario workloads')
     ap.add_argument('--out', default=None)
     a = ap.parse_args()
     import torch
     if not torch.cuda.is_available():
         raise SystemExit('freet_mpc_bench.py needs a CUDA device')
     res = {'card': card(), 'device': torch.cuda.get_device_name(0), 'update_time': DT, 'runs': []}
-    for name, batch, kw in WORKLOADS:
+    workloads = [(name, a.batch, {}) for name in a.scenario] if a.scenario else WORKLOADS
+    for name, batch, kw in workloads:
         res['runs'].append(one_run(name, batch, kw, a.steps, a.closed))
     line = json.dumps(res)
     print(line)
     if a.out:
         os.makedirs(a.out, exist_ok=True)
-        fn = 'freet_mpc_bench_closed.json' if a.closed else 'freet_mpc_bench.json'
+        fn = 'freet_mpc_bench%s%s.json' % ('_' + '_'.join(a.scenario) if a.scenario else '',
+                                           '_closed' if a.closed else '')
         with open(os.path.join(a.out, fn), 'w') as f:
             f.write(line + '\n')
 
