@@ -484,6 +484,101 @@ int omg_admm_zl_update_dist(omg_comm* c, int32_t n_local, int32_t nsh, int32_t n
 omg_tables* omg_tables_read(const char* path);
 void omg_tables_free(omg_tables* tables);
 
+/* ---- device-resident receding-horizon update ------------------------------------------------
+ * The batched counterpart of the reference's exported Point2Point::update()
+ * (omgtools/export/point2point/Point2Point.cpp:119-231) for a fixed-horizon Point2point with one
+ * Holonomic or Holonomic3D vehicle (n_dim position splines; state = their values, input = their
+ * derivatives / horizon) and obstacles that are static, move with x/v/a or rotate with theta.
+ * One omg_mpc_update advances B independent instances, each on its own time t_b (B copies of
+ * Point2Point), stream-ordered: after the first update of a handle it makes no synchronous CUDA
+ * call and no allocation, so a sequence of updates can be captured in a CUDA graph.
+ *
+ * Per instance b, with round6(x) = rint(x * 1e6) / 1e6 (numpy.round(x, 6)), t_rel = round6(t_b)
+ * mod knot_time, and a knot crossed when trunc(round6(t_prev_b / knot_time)) <
+ * trunc(round6(t_b / knot_time)):
+ *   prepare  cold start when |t_b| <= 1e-6 or the instance was flagged by omg_mpc_recover:
+ *            state0 = the caller's state0[b], input0 = 0 (Holonomic::setInitialConditions), and
+ *            the x row is x_template with the vehicle's columns set to linspace(state0, stateT, L)
+ *            (getInitSplineValue).  Otherwise the prediction made when the last successful plan
+ *            was committed: ideal: the plan's value and derivative / horizon at
+ *            t_rel_prev + update_time; integrate: classical RK4 from the caller's state0[b]
+ *            (the measured state at the start of that plan) over the plan's inputs at the
+ *            update_time / sample_time + 1 samples from t_rel_prev, on the linearly interpolated
+ *            input (the integration of omg_closed_loop_step's predict half, which is what the
+ *            reference's Python predict does with odeint; Vehicle.cpp's predict takes the stage
+ *            inputs instead), input0 = the planned input at the last sample.  At a knot crossing
+ *            every shift block is multiplied by its T matrix (omg_shift_batch).  P[b] is
+ *            p_template with state0, input0, poseT = stateT[b], t = t_rel, T = horizon and the
+ *            obstacles' x, v, a (and theta) written in.
+ *   solve    omg_solve_batch with the problem's own bounds, shared by all instances.
+ *   commit   status 0: the x row takes the solution, t_prev_b = t_b, state_traj[b] and
+ *            input_traj[b] receive the plan's values and derivatives / horizon at
+ *            t_rel + k * sample_time (k < trajectory_length; a sample past the horizon reads 0),
+ *            the next prediction is stored and t_b = round6(t_b + update_time).  Any other
+ *            status: t_prev_b = t_b (the next update does not shift again), the x row keeps the
+ *            warm start it was solved from, t_b and the output rows are left as they were
+ *            (Point2Point::update returns false).  status[b] and iters[b] are always written.
+ * Obstacles are supplied on every call in their current state (the reference's obstacle_t):
+ * obstacles[b] holds n_obs records of 3 * n_dim + 1 doubles, {x, v, a, theta}; theta is read only
+ * for a rotating obstacle.  Not covered: a free horizon, several vehicles, other vehicles, run-time
+ * bounds (updateBounds), predict_shift and provide_prediction. */
+typedef struct omg_mpc omg_mpc;   /* opaque handle */
+
+typedef struct omg_mpc_desc {
+  int32_t n, n_par;               /* the problem's sizes */
+  int32_t n_dim;                  /* vehicle: states = inputs = position splines, 1 .. 3 */
+  int32_t spl_offset;             /* column c of the vehicle's splines at x[spl_offset + c * L] */
+  int32_t L, degree;              /* the vehicle's B-spline basis on [0, 1] */
+  const double* knots;            /* [L + degree + 1] */
+  double horizon, knot_time, update_time, sample_time;
+  int32_t p_state0, p_input0, p_poseT, p_t, p_T;   /* offsets in p */
+  int32_t n_obs;
+  const int32_t* obs_kind;        /* [n_obs] 0: x, v, a; 1: x, v, a and theta (rotating) */
+  const int32_t* obs_off;         /* [n_obs * 4] offsets in p of x, v, a, theta (-1: none) */
+  int32_t n_shift;                /* warm-start shift blocks (father.shifted_entries()) */
+  const int32_t* shift_off;       /* [n_shift] offset in x */
+  const int32_t* shift_len;       /* [n_shift] basis length len */
+  const int32_t* shift_ncol;      /* [n_shift] columns */
+  const double* shift_T;          /* the n_shift row-major len x len matrices, concatenated */
+  const double* x_template;       /* [n] father.get_variables().cat */
+  const double* p_template;       /* [n_par] father.set_parameters(0.).cat */
+} omg_mpc_desc;
+
+enum { OMG_MPC_PREDICT_IDEAL = 0, OMG_MPC_PREDICT_INTEGRATE = 1 };
+
+/* MPC files: "OMGMPC\0\0", int32 abi_version, int32 record count, then records in the format of
+ * the table file, named after the fields of omg_mpc_desc (float64 scalars as records of one
+ * double).  Written by omg_tools_b200.solver.b200.save_mpc.  omg_mpc_read returns a heap object
+ * that owns its arrays (release it with omg_mpc_free_desc) or NULL (omg_last_error). */
+omg_mpc_desc* omg_mpc_read(const char* path);
+void omg_mpc_free_desc(omg_mpc_desc* desc);
+
+/* Allocate the loop's state for B instances of `problem` on its device (the handle keeps a
+ * pointer to the problem, which must outlive it).  prediction: OMG_MPC_PREDICT_*.  Returns NULL
+ * with a message for: a null argument, n or n_par that differ from the problem's, B <= 0,
+ * trajectory_length < 1 or above horizon / sample_time, an update_time that is not a positive
+ * multiple of sample_time, an unknown prediction, and descriptor entries outside x or p. */
+omg_mpc* omg_mpc_create(omg_problem* problem, const omg_mpc_desc* desc, int32_t B,
+                        int32_t trajectory_length, int32_t prediction);
+void omg_mpc_destroy(omg_mpc* mpc);
+
+/* One update of every instance (see above).  DEVICE buffers: state0, stateT [B][n_dim],
+ * obstacles [B][n_obs][3 n_dim + 1] (may be NULL when n_obs = 0), state_traj, input_traj
+ * [B][trajectory_length][n_dim], status, iters [B].  Asynchronous on `stream`. */
+int omg_mpc_update(omg_mpc* mpc, const double* state0, const double* stateT, const double* obstacles,
+                   double* state_traj, double* input_traj, int32_t* status, int32_t* iters, void* stream);
+/* Same call with HOST buffers (synchronous). */
+int omg_mpc_update_host(omg_mpc* mpc, const double* state0, const double* stateT, const double* obstacles,
+                        double* state_traj, double* input_traj, int32_t* status, int32_t* iters);
+/* Cold-start the instances with mask[b] != 0 (HOST int32 [B]) on their next update, as
+ * Point2Point::recover().  Synchronous: the flags are set when the call returns. */
+int omg_mpc_recover(omg_mpc* mpc, const int32_t* mask);
+/* Current time t_b of every instance into HOST t_out [B] (synchronises the device). */
+int omg_mpc_time(omg_mpc* mpc, double* t_out);
+/* The warm start and parameter rows handed to the last solve, DEVICE x0_out [B][n] and p_out
+ * [B][n_par] (either may be NULL).  Asynchronous on `stream`. */
+int omg_mpc_last_problem(omg_mpc* mpc, double* x0_out, double* p_out, void* stream);
+
 const char* omg_last_error(void);
 int omg_abi_version(void);
 

@@ -1236,6 +1236,18 @@ omg_ipm_kernel_xl(const DevTab T, const omg_options O, const Batch A, const Smem
 template <bool WIDE> __global__ void __launch_bounds__(256, 2)
 omg_ipm_kernel_xl_2cta(const DevTab T, const omg_options O, const Batch A, const Smem S) { ipm_body<true, WIDE>(T, O, A, S); }
 
+// one shift block (offset off, basis length L, nc columns) of one instance, spread over the threads
+// of a block: dst[off + c*L + i] = sum_k T[i,k] src[off + c*L + k] (src must not alias dst)
+__device__ __forceinline__ void omg_shift_block(const double* Tb, const double* src, double* dst, int off, int L,
+                                                int nc) {
+  for (int e = threadIdx.x; e < L * nc; e += blockDim.x) {
+    const int c = e / L, i = e % L;
+    double acc = 0.0;
+    for (int k = 0; k < L; ++k) acc += Tb[i * L + k] * src[off + c * L + k];
+    dst[off + c * L + i] = acc;
+  }
+}
+
 // warm-start shift: x[b, off + c*len + i] <- sum_k T[i,k] x[b, off + c*len + k]
 __global__ void omg_shift_kernel(double* x, int B, int n, int n_blocks, const int* offs,
                                  const int* lens, const int* ncols, const int* toffs,
@@ -1249,12 +1261,7 @@ __global__ void omg_shift_kernel(double* x, int B, int n, int n_blocks, const in
   for (int blk = 0; blk < n_blocks; ++blk) {
     const int L = lens[blk], nc = ncols[blk], off = offs[blk];
     const double* Tb = Tm + toffs[blk];
-    for (int e = threadIdx.x; e < L * nc; e += blockDim.x) {
-      const int c = e / L, i = e % L;
-      double acc = 0.0;
-      for (int k = 0; k < L; ++k) acc += Tb[i * L + k] * xs[off + c * L + k];
-      xb[off + c * L + i] = acc;
-    }
+    omg_shift_block(Tb, xs, xb, off, L, nc);
   }
 }
 
@@ -1393,6 +1400,28 @@ __device__ __forceinline__ void omg_cl_input_map(int model, int ni, const double
   }
 }
 
+// Classical RK4 of the vehicle ODE from the state y over the n_samp sample intervals of the input
+// samples U [n_samp+1][ni] on the linearly interpolated input of the reference's interp1d: u_i,
+// the mean of u_i and u_i+1 at both midpoints, u_i+1 at the end.  y is updated in place.  The work
+// arrays st, k1..k4 [OMG_ODE_MAX_STATE] and um [OMG_CL_MAX_INPUT] are the caller's.
+__device__ __forceinline__ void omg_rk4_interp(int ode, int ns, int ni, int n_samp, double dt, const double* U,
+                                               double* y, double* st, double* k1, double* k2, double* k3,
+                                               double* k4, double* um) {
+  for (int i = 0; i < n_samp; ++i) {
+    const double* u0 = U + i * ni;
+    const double* u1 = u0 + ni;
+    for (int c = 0; c < ni; ++c) um[c] = 0.5 * (u0[c] + u1[c]);
+    ode_rhs(ode, ns, y, u0, k1);
+    for (int j = 0; j < ns; ++j) st[j] = y[j] + 0.5 * dt * k1[j];
+    ode_rhs(ode, ns, st, um, k2);
+    for (int j = 0; j < ns; ++j) st[j] = y[j] + 0.5 * dt * k2[j];
+    ode_rhs(ode, ns, st, um, k3);
+    for (int j = 0; j < ns; ++j) st[j] = y[j] + dt * k3[j];
+    ode_rhs(ode, ns, st, u1, k4);
+    for (int j = 0; j < ns; ++j) y[j] += (dt / 6.0) * (k1[j] + 2.0 * k2[j] + 2.0 * k3[j] + k4[j]);
+  }
+}
+
 // The part of one instance's plant step that follows the planned inputs U [n_samp+1][ni] (shared
 // memory, complete at entry or completed by the caller's threads before the barrier below), run
 // by every thread of the block:
@@ -1472,19 +1501,7 @@ __device__ void omg_cl_tail(int b, int p, int sig0, int ode, int ns, int ni, int
     }
     Uin = A;
   }
-  for (int i = 0; i < n_samp; ++i) {
-    const double* u0 = Uin + i * ni;
-    const double* u1 = u0 + ni;
-    for (int c = 0; c < ni; ++c) um[c] = 0.5 * (u0[c] + u1[c]);
-    ode_rhs(ode, ns, y, u0, k1);
-    for (int j = 0; j < ns; ++j) st[j] = y[j] + 0.5 * dt * k1[j];
-    ode_rhs(ode, ns, st, um, k2);
-    for (int j = 0; j < ns; ++j) st[j] = y[j] + 0.5 * dt * k2[j];
-    ode_rhs(ode, ns, st, um, k3);
-    for (int j = 0; j < ns; ++j) st[j] = y[j] + dt * k3[j];
-    ode_rhs(ode, ns, st, u1, k4);
-    for (int j = 0; j < ns; ++j) y[j] += (dt / 6.0) * (k1[j] + 2.0 * k2[j] + 2.0 * k3[j] + k4[j]);
-  }
+  omg_rk4_interp(ode, ns, ni, n_samp, dt, Uin, y, st, k1, k2, k3, k4, um);
   double* xo = simulate ? plant_x_next : pred_x;
   double* uo = simulate ? plant_u_next : pred_u;
   for (int j = 0; j < ns; ++j) xo[(size_t)p * ns + j] = y[j];
@@ -1702,6 +1719,19 @@ __global__ void omg_shift_free_kernel(double* x, int B, int n, int t_index, doub
   }
   __syncthreads();                                // (every thread has read T)
   if (t == 0) xb[t_index] = target;
+}
+
+// Derivative coefficients of one spline column c [L] of degree p on the knots k, the arithmetic of
+// omg_eval_kernel and omg_closed_loop_free_kernel (which keep their own inline copies: routed through
+// this function, their generated code changes): row d of q [n_der][L] holds the L - d coefficients
+// of the d-th derivative.
+__device__ __forceinline__ void omg_spl_der_coef(const double* k, int p, int L, int n_der, const double* c, double* q) {
+  for (int i = 0; i < L; ++i) q[i] = c[i];
+  for (int d = 1; d < n_der; ++d)
+    for (int j = 0; j < L - d; ++j) {
+      const double den = k[j + p + 1] - k[j + d];
+      q[d * L + j] = den != 0.0 ? (p - d + 1) * (q[(d - 1) * L + j + 1] - q[(d - 1) * L + j]) / den : 0.0;
+    }
 }
 
 // Per-instance evaluation, one instance per block: out[b, blk, c, j, d] = d-th derivative of
@@ -2111,6 +2141,7 @@ struct omg_problem {
   // scratch of the feasibility phase (omg_feas_batch), sized on first use
   double* fscr = nullptr; int fscr_ctas = 0; size_t fscr_stride = 0;
   DescCache* shift_desc = nullptr;   // device copy of the last omg_shift_batch block descriptor
+  const double* lbg = nullptr; const double* ubg = nullptr;   // the tables' bounds (omg_mpc_update)
   // sparse kernel variant (omg_sp.cuh / omg_sp_host.cuh)
   bool sp = false; SpTab P; SpSmem SS; size_t sp_smem_bytes = 0; int sp_ctas = 0, sp_dscr_stride = 0;
   std::string sp_info, sp_info_extra;
@@ -2280,6 +2311,8 @@ omg_problem* omg_problem_create(const omg_tables* tb, const omg_options* opt, in
       set_err("envelope rows must start at multiples of the panel width"); ok = false; }
   if (!ok) { delete h; return nullptr; }
 
+  h->lbg = upload(h, tb->lbg, m, &ok);
+  h->ubg = upload(h, tb->ubg, m, &ok);
   T.tape_func = upload(h, tb->tape_func, tb->n_tape, &ok);
   T.tape_ptr = upload(h, tb->tape_ptr, (size_t)tb->n_tape + 1, &ok);
   T.tape_coef = upload(h, tb->tape_coef, tb->n_tape_terms, &ok);
@@ -3271,6 +3304,448 @@ int omg_admm_zl_update_dist(omg_comm* c, int32_t n_local, int32_t nsh, int32_t n
   OMG_LAUNCH(omg_gather_rows_kernel, n_local * n_nghb, 32, 0, stream, n_local * n_nghb, nsh, n_nghb * nsh, nghb, back, allz, z_ji);
   OMG_LAUNCH(omg_gather_rows_kernel, n_local * n_nghb, 32, 0, stream, n_local * n_nghb, nsh, n_nghb * nsh, nghb, back, alll, l_ji);
   CK(cudaGetLastError());
+  return 0;
+}
+
+}  // extern "C"
+
+// ===========================================================================
+// Device-resident receding-horizon update (include/omg_b200.h: omg_mpc_*), the batched
+// Point2Point::update() of the reference's export (Point2Point.cpp:119-231) for one Holonomic /
+// Holonomic3D vehicle with a fixed horizon.  Two kernels around omg_solve_batch, one instance
+// per block: prepare (cold start or knot shift, prediction, parameter row) and commit (accept or
+// keep, trajectory samples, the next prediction).
+// ===========================================================================
+struct MpcDev {
+  int B, n, n_par, nd, spl_off, L, p, traj_len, n_samp, mode, n_obs, n_shift;
+  int p_state0, p_input0, p_poseT, p_t, p_T;
+  double horizon, knot_time, update_time, sample_time;
+  const double* knots;      // [L + p + 1]
+  const int* obs_kind;      // [n_obs]
+  const int* obs_off;       // [n_obs][4]
+  const int* shift_desc;    // [n_shift][4]: offset in x, len, columns, offset of its T in shift_T
+  const double* shift_T;
+  const double* x_tpl;      // [n]
+  const double* p_tpl;      // [n_par]
+  double* X;                // [B][n] the warm start of the next update (last accepted solution)
+  double* X0;               // [B][n] the warm start handed to the solve
+  double* Xn;               // [B][n] the solve's result
+  double* P;                // [B][n_par]
+  double* t;                // [B] instance time
+  double* t_prev;           // [B]
+  double* pred_x;           // [B][nd] ideal prediction: state at t_rel + update_time
+  double* pred_u;           // [B][nd] and input
+  double* U;                // [B][n_samp + 1][nd] integrate: planned inputs from t_rel
+  int* rec;                 // [B] cold start requested by omg_mpc_recover
+};
+
+// numpy.round(x, 6)
+__device__ __forceinline__ double omg_round6(double x) { return rint(x * 1e6) / 1e6; }
+
+// Shared memory: source x row [n] | warm start [n].
+__global__ void omg_mpc_prepare_kernel(const MpcDev M, const double* __restrict__ state0,
+                                       const double* __restrict__ stateT, const double* __restrict__ obs) {
+  OMG_DYN_SHARED(xs);
+  const int b = blockIdx.x, t = threadIdx.x, nt = blockDim.x, n = M.n, nd = M.nd, L = M.L;
+  if (b >= M.B) return;
+  double* ws = xs + n;
+  const double tb = M.t[b], kt = M.knot_time;
+  const bool cold = fabs(tb) <= 1e-6 || M.rec[b] != 0;
+  const bool cross = !cold && (long long)omg_round6(M.t_prev[b] / kt) < (long long)omg_round6(tb / kt);
+  const double* src = cold ? M.x_tpl : M.X + (size_t)b * n;
+  for (int i = t; i < n; i += nt) xs[i] = ws[i] = src[i];
+  __syncthreads();
+  if (cold) {                         // getInitSplineValue: linspace(state0, stateT, L) per column
+    for (int e = t; e < nd * L; e += nt) {
+      const int c = e / L, i = e - c * L;
+      ws[M.spl_off + e] = omg_linspace(state0[(size_t)b * nd + c], stateT[(size_t)b * nd + c], L, i);
+    }
+  } else if (cross) {                 // transformSplines
+    for (int k = 0; k < M.n_shift; ++k) {
+      const int* d = M.shift_desc + 4 * k;
+      omg_shift_block(M.shift_T + d[3], xs, ws, d[0], d[1], d[2]);
+    }
+  }
+  __syncthreads();
+  double* x0 = M.X0 + (size_t)b * n;
+  double* pb = M.P + (size_t)b * M.n_par;
+  for (int i = t; i < n; i += nt) x0[i] = ws[i];
+  for (int i = t; i < M.n_par; i += nt) pb[i] = M.p_tpl[i];
+  __syncthreads();                    // (the template row is in place; every thread has read rec[b])
+  if (t != 0) return;
+  double s0[OMG_ODE_MAX_STATE], u0[OMG_CL_MAX_INPUT];
+  const double* st0 = state0 + (size_t)b * nd;
+  if (cold) {                         // Holonomic::setInitialConditions
+    for (int c = 0; c < nd; ++c) { s0[c] = st0[c]; u0[c] = 0.0; }
+  } else if (M.mode == OMG_MPC_PREDICT_IDEAL) {
+    for (int c = 0; c < nd; ++c) { s0[c] = M.pred_x[(size_t)b * nd + c]; u0[c] = M.pred_u[(size_t)b * nd + c]; }
+  } else {                            // RK4 from the measured state over the planned inputs
+    const double* Ub = M.U + (size_t)b * (M.n_samp + 1) * nd;
+    for (int c = 0; c < nd; ++c) s0[c] = st0[c];
+    double st[OMG_ODE_MAX_STATE], k1[OMG_ODE_MAX_STATE], k2[OMG_ODE_MAX_STATE], k3[OMG_ODE_MAX_STATE],
+           k4[OMG_ODE_MAX_STATE], um[OMG_CL_MAX_INPUT];
+    omg_rk4_interp(OMG_ODE_INTEGRATOR, nd, nd, M.n_samp, M.sample_time, Ub, s0, st, k1, k2, k3, k4, um);
+    for (int c = 0; c < nd; ++c) u0[c] = Ub[(size_t)M.n_samp * nd + c];
+  }
+  for (int c = 0; c < nd; ++c) {
+    pb[M.p_state0 + c] = s0[c];
+    pb[M.p_input0 + c] = u0[c];
+    pb[M.p_poseT + c] = stateT[(size_t)b * nd + c];
+  }
+  pb[M.p_t] = fmod(omg_round6(tb), kt);
+  pb[M.p_T] = M.horizon;
+  const int rl = 3 * nd + 1;
+  for (int k = 0; k < M.n_obs; ++k) {
+    const double* o = obs + ((size_t)b * M.n_obs + k) * rl;
+    const int* off = M.obs_off + 4 * k;
+    for (int c = 0; c < nd; ++c) {
+      pb[off[0] + c] = o[c];
+      pb[off[1] + c] = o[nd + c];
+      pb[off[2] + c] = o[2 * nd + c];
+    }
+    if (M.obs_kind[k]) pb[off[3]] = o[3 * nd];
+  }
+  M.rec[b] = 0;
+}
+
+// Shared memory: the derivative coefficients (value and first derivative) of the vehicle's columns
+// [nd][2][L] (omg_spl_der_coef).  Sample j < traj_len is the output row j; the samples after them
+// are the next prediction's: one point at t_rel + update_time (ideal) or n_samp + 1 points at
+// t_rel + s * sample_time (integrate).
+__global__ void omg_mpc_commit_kernel(const MpcDev M, const int* __restrict__ status, double* __restrict__ state_traj,
+                                      double* __restrict__ input_traj) {
+  OMG_DYN_SHARED(cd);
+  const int b = blockIdx.x, t = threadIdx.x, nt = blockDim.x, n = M.n, nd = M.nd, L = M.L, p = M.p;
+  if (b >= M.B) return;
+  const bool ok = status[b] == 0;
+  const double tb = M.t[b];
+  const double* src = (ok ? M.Xn : M.X0) + (size_t)b * n;
+  double* xb = M.X + (size_t)b * n;
+  for (int i = t; i < n; i += nt) xb[i] = src[i];
+  if (!ok) {                          // keep the warm start and the time; do not shift again
+    if (t == 0) M.t_prev[b] = tb;
+    return;
+  }
+  for (int c = t; c < nd; c += nt) omg_spl_der_coef(M.knots, p, L, 2, src + M.spl_off + c * L, cd + (size_t)c * 2 * L);
+  __syncthreads();
+  const double t_rel = fmod(omg_round6(tb), M.knot_time), T = M.horizon;
+  const bool ideal = M.mode == OMG_MPC_PREDICT_IDEAL;
+  const int tl = M.traj_len, n_pts = tl + (ideal ? 1 : M.n_samp + 1);
+  for (int j = t; j < n_pts; j += nt) {
+    const double tau = j < tl ? (t_rel + (double)j * M.sample_time) / T
+                       : ideal ? (t_rel + M.update_time) / T : (t_rel + (double)(j - tl) * M.sample_time) / T;
+    double w[OMG_SPL_MAX_LEN + OMG_SPL_MAX_DEGREE], v[2][OMG_CL_MAX_INPUT];
+    for (int d = 0; d < 2; ++d) {
+      omg_cox_de_boor(M.knots + d, p - d, tau, 0, L - d, w);
+      for (int c = 0; c < nd; ++c) {
+        const double* q = cd + ((size_t)c * 2 + d) * L;
+        double acc = 0.0;
+        for (int i = 0; i < L - d; ++i) acc += w[i] * q[i];
+        v[d][c] = d ? acc / T : acc;
+      }
+    }
+    double *xo, *uo;
+    if (j < tl) {
+      xo = state_traj + ((size_t)b * tl + j) * nd;
+      uo = input_traj + ((size_t)b * tl + j) * nd;
+    } else if (ideal) {
+      xo = M.pred_x + (size_t)b * nd;
+      uo = M.pred_u + (size_t)b * nd;
+    } else {
+      xo = nullptr;
+      uo = M.U + ((size_t)b * (M.n_samp + 1) + (j - tl)) * nd;
+    }
+    for (int c = 0; c < nd; ++c) {
+      if (xo) xo[c] = v[0][c];
+      uo[c] = v[1][c];
+    }
+  }
+  __syncthreads();                    // (every thread has read t_b)
+  if (t == 0) {
+    M.t_prev[b] = tb;
+    M.t[b] = omg_round6(tb + M.update_time);
+  }
+}
+
+__global__ void omg_mpc_flag_kernel(int B, const int* __restrict__ mask, int* __restrict__ rec) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b < B && mask[b]) rec[b] = 1;
+}
+
+#define OMG_MPC_NT 128
+
+struct omg_mpc {
+  omg_problem* h = nullptr;
+  MpcDev M;
+  size_t smem_prepare = 0, smem_commit = 0;
+  std::vector<void*> allocs;
+  double* lam = nullptr; double* f = nullptr;
+  int* mask = nullptr;
+  // device staging of omg_mpc_update_host
+  double *s0 = nullptr, *sT = nullptr, *obs = nullptr, *xtraj = nullptr, *utraj = nullptr;
+  int *st = nullptr, *it = nullptr;
+};
+
+namespace {
+// fields of an MPC file: kind 0 int32 scalar, 1 float64 scalar, 2 int32 array, 3 float64 array
+struct MpcField { const char* name; int kind; size_t off; };
+#define MF(f, k) {#f, k, offsetof(omg_mpc_desc, f)}
+const MpcField kMpcFields[] = {
+  MF(n, 0), MF(n_par, 0), MF(n_dim, 0), MF(spl_offset, 0), MF(L, 0), MF(degree, 0), MF(knots, 3),
+  MF(horizon, 1), MF(knot_time, 1), MF(update_time, 1), MF(sample_time, 1),
+  MF(p_state0, 0), MF(p_input0, 0), MF(p_poseT, 0), MF(p_t, 0), MF(p_T, 0),
+  MF(n_obs, 0), MF(obs_kind, 2), MF(obs_off, 2),
+  MF(n_shift, 0), MF(shift_off, 2), MF(shift_len, 2), MF(shift_ncol, 2), MF(shift_T, 3),
+  MF(x_template, 3), MF(p_template, 3),
+};
+#undef MF
+struct OwnedMpc { omg_mpc_desc D; std::vector<void*> blocks; };
+
+bool mpc_range(const std::string& what, int64_t lo, int64_t len, int64_t size) {
+  if (lo < 0 || len < 0 || lo + len > size) {
+    set_err("omg_mpc_create: " + what + " at " + std::to_string(lo) + " (+" + std::to_string(len) + ") outside [0, " +
+            std::to_string(size) + ")");
+    return false;
+  }
+  return true;
+}
+
+// Checks of omg_mpc_create; n_samp receives update_time / sample_time.
+bool mpc_check(const omg_problem* h, const omg_mpc_desc* D, int32_t B, int32_t traj_len, int32_t mode, int* n_samp) {
+  const std::string f("omg_mpc_create: ");
+  if (D->n != h->T.n || D->n_par != h->T.n_par) {
+    set_err(f + "the descriptor is for n = " + std::to_string(D->n) + ", n_par = " + std::to_string(D->n_par) +
+            ", the problem has n = " + std::to_string(h->T.n) + ", n_par = " + std::to_string(h->T.n_par));
+    return false;
+  }
+  if (B <= 0) { set_err(f + "B must be >= 1, got " + std::to_string(B)); return false; }
+  if (mode != OMG_MPC_PREDICT_IDEAL && mode != OMG_MPC_PREDICT_INTEGRATE) {
+    set_err(f + "unknown prediction " + std::to_string(mode)); return false; }
+  if (!(D->horizon > 0.0) || !(D->knot_time > 0.0) || !(D->sample_time > 0.0) || !(D->update_time > 0.0)) {
+    set_err(f + "horizon, knot_time, update_time and sample_time must be > 0"); return false; }
+  const double r = D->update_time / D->sample_time;
+  *n_samp = (int)rint(r);
+  if (*n_samp < 1 || fabs(r - *n_samp) > 1e-9 * std::max(1.0, r)) {
+    set_err(f + "update_time " + std::to_string(D->update_time) + " is not a multiple of sample_time " +
+            std::to_string(D->sample_time)); return false; }
+  const int max_len = (int)rint(D->horizon / D->sample_time * 1e6) / 1000000;
+  if (traj_len < 1 || traj_len > max_len) {
+    set_err(f + "trajectory_length " + std::to_string(traj_len) + " outside 1 .. horizon / sample_time = " +
+            std::to_string(max_len)); return false; }
+  const int nd = D->n_dim, L = D->L, p = D->degree;
+  if (nd < 1 || nd > OMG_CL_MAX_INPUT) { set_err(f + "n_dim must be 1 .. 3"); return false; }
+  if (p < 1 || p > OMG_SPL_MAX_DEGREE || L < p + 1 || L > OMG_SPL_MAX_LEN) {
+    set_err(f + "degree " + std::to_string(p) + " / basis length " + std::to_string(L) + " outside 1 <= p <= " +
+            std::to_string(OMG_SPL_MAX_DEGREE) + ", p + 1 <= L <= " + std::to_string(OMG_SPL_MAX_LEN)); return false; }
+  if (!D->knots || !D->x_template || !D->p_template || (D->n_obs > 0 && (!D->obs_kind || !D->obs_off)) ||
+      (D->n_shift > 0 && (!D->shift_off || !D->shift_len || !D->shift_ncol || !D->shift_T)) ||
+      D->n_obs < 0 || D->n_shift < 0) { set_err(f + "null descriptor array"); return false; }
+  for (int j = 0; j < L + p; ++j)
+    if (!(D->knots[j] <= D->knots[j + 1])) { set_err(f + "knots not non-decreasing"); return false; }
+  if (!mpc_range("vehicle splines", D->spl_offset, (int64_t)nd * L, D->n) ||
+      !mpc_range("state0", D->p_state0, nd, D->n_par) || !mpc_range("input0", D->p_input0, nd, D->n_par) ||
+      !mpc_range("poseT", D->p_poseT, nd, D->n_par) || !mpc_range("t", D->p_t, 1, D->n_par) ||
+      !mpc_range("T", D->p_T, 1, D->n_par)) return false;
+  for (int k = 0; k < D->n_obs; ++k) {
+    const std::string o = "obstacle " + std::to_string(k) + " ";
+    if (D->obs_kind[k] != 0 && D->obs_kind[k] != 1) { set_err(f + o + "kind must be 0 or 1"); return false; }
+    for (int q = 0; q < 3; ++q)
+      if (!mpc_range(o + "x/v/a", D->obs_off[4 * k + q], nd, D->n_par)) return false;
+    if (D->obs_kind[k] && !mpc_range(o + "theta", D->obs_off[4 * k + 3], 1, D->n_par)) return false;
+  }
+  for (int k = 0; k < D->n_shift; ++k)
+    if (D->shift_len[k] < 1 || D->shift_ncol[k] < 1 ||
+        !mpc_range("shift block " + std::to_string(k), D->shift_off[k], (int64_t)D->shift_len[k] * D->shift_ncol[k], D->n))
+      return false;
+  if (2 * (size_t)D->n * sizeof(double) > 227 * 1024) { set_err(f + "two x rows exceed the shared memory of a block"); return false; }
+  return true;
+}
+}  // namespace
+
+extern "C" {
+
+omg_mpc_desc* omg_mpc_read(const char* path) {
+  FILE* fp = path ? fopen(path, "rb") : nullptr;
+  if (!fp) { set_err(std::string("cannot open MPC file ") + (path ? path : "(null)")); return nullptr; }
+  OwnedMpc* O = new OwnedMpc();
+  memset(&O->D, 0, sizeof(O->D));
+  bool ok = true;
+  char magic[8]; int32_t ver = 0, nrec = 0;
+  if (fread(magic, 1, 8, fp) != 8 || memcmp(magic, "OMGMPC\0\0", 8) != 0) { set_err("not an omg MPC file"); ok = false; }
+  if (ok && (fread(&ver, 4, 1, fp) != 1 || fread(&nrec, 4, 1, fp) != 1)) { set_err("truncated MPC file"); ok = false; }
+  if (ok && ver != OMG_ABI_VERSION) { set_err("MPC file written for another ABI version"); ok = false; }
+  const int nf = (int)(sizeof(kMpcFields) / sizeof(kMpcFields[0]));
+  std::vector<char> seen(nf, 0);
+  for (int r = 0; ok && r < nrec; ++r) {
+    char name[24]; int32_t dtype = 0, pad = 0; int64_t count = 0;
+    if (fread(name, 1, 24, fp) != 24 || fread(&dtype, 4, 1, fp) != 1 || fread(&pad, 4, 1, fp) != 1 ||
+        fread(&count, 8, 1, fp) != 1 || count < 0) { set_err("truncated MPC file"); ok = false; break; }
+    name[23] = 0;
+    int k = -1;
+    for (int q = 0; q < nf; ++q) if (strcmp(kMpcFields[q].name, name) == 0) { k = q; break; }
+    const int kind = k < 0 ? -1 : kMpcFields[k].kind;
+    if (k < 0 || dtype != (kind == 1 || kind == 3 ? 1 : 0)) { set_err(std::string("unknown record in MPC file: ") + name); ok = false; break; }
+    const size_t esz = dtype ? 8 : 4;
+    char* base = reinterpret_cast<char*>(&O->D) + kMpcFields[k].off;
+    if (kind < 2) {
+      if (count != 1 || fread(base, esz, 1, fp) != 1) { set_err(std::string("bad scalar record ") + name); ok = false; break; }
+    } else {
+      void* blk = malloc((size_t)(count > 0 ? count : 1) * esz);
+      O->blocks.push_back(blk);
+      if (!blk || (count > 0 && fread(blk, esz, (size_t)count, fp) != (size_t)count)) { set_err("truncated MPC file"); ok = false; break; }
+      *reinterpret_cast<void**>(base) = blk;
+    }
+    seen[k] = 1;
+  }
+  fclose(fp);
+  for (int q = 0; ok && q < nf; ++q)
+    if (!seen[q]) { set_err(std::string("MPC file lacks ") + kMpcFields[q].name); ok = false; }
+  if (!ok) { omg_mpc_free_desc(&O->D); return nullptr; }
+  return &O->D;
+}
+
+void omg_mpc_free_desc(omg_mpc_desc* desc) {
+  if (!desc) return;
+  OwnedMpc* O = reinterpret_cast<OwnedMpc*>(desc);   // D is the first member
+  for (void* b : O->blocks) free(b);
+  delete O;
+}
+
+void omg_mpc_destroy(omg_mpc* mpc) {
+  if (!mpc) return;
+  cudaSetDevice(mpc->h->device);
+  for (void* p : mpc->allocs) cudaFree(p);
+  delete mpc;
+}
+
+omg_mpc* omg_mpc_create(omg_problem* h, const omg_mpc_desc* D, int32_t B, int32_t traj_len, int32_t mode) {
+  if (!h || !D) { set_err("omg_mpc_create: null argument"); return nullptr; }
+  int n_samp = 0;
+  if (!mpc_check(h, D, B, traj_len, mode, &n_samp)) return nullptr;
+  if (cudaSetDevice(h->device) != cudaSuccess) { set_err("omg_mpc_create: cudaSetDevice failed"); return nullptr; }
+  omg_mpc* q = new omg_mpc();
+  q->h = h;
+  MpcDev& M = q->M;
+  memset(&M, 0, sizeof(M));
+  const int n = D->n, np_ = D->n_par, nd = D->n_dim, L = D->L, p = D->degree;
+  M.B = B; M.n = n; M.n_par = np_; M.nd = nd; M.spl_off = D->spl_offset; M.L = L; M.p = p;
+  M.traj_len = traj_len; M.n_samp = n_samp; M.mode = mode; M.n_obs = D->n_obs; M.n_shift = D->n_shift;
+  M.p_state0 = D->p_state0; M.p_input0 = D->p_input0; M.p_poseT = D->p_poseT; M.p_t = D->p_t; M.p_T = D->p_T;
+  M.horizon = D->horizon; M.knot_time = D->knot_time; M.update_time = D->update_time; M.sample_time = D->sample_time;
+  bool ok = true;
+  auto alloc = [&](size_t bytes, const void* src) -> void* {
+    void* d = nullptr;
+    if (cudaMalloc(&d, bytes ? bytes : 8) != cudaSuccess) { ok = false; return nullptr; }
+    q->allocs.push_back(d);
+    if (src && bytes && cudaMemcpy(d, src, bytes, cudaMemcpyHostToDevice) != cudaSuccess) ok = false;
+    else if (!src && cudaMemset(d, 0, bytes ? bytes : 8) != cudaSuccess) ok = false;
+    return d;
+  };
+  std::vector<int> sd(4 * (size_t)D->n_shift);
+  size_t nT = 0;
+  for (int k = 0; k < D->n_shift; ++k) {
+    sd[4 * k] = D->shift_off[k]; sd[4 * k + 1] = D->shift_len[k]; sd[4 * k + 2] = D->shift_ncol[k]; sd[4 * k + 3] = (int)nT;
+    nT += (size_t)D->shift_len[k] * D->shift_len[k];
+  }
+  const size_t b = B, d8 = sizeof(double);
+  M.knots = (const double*)alloc(d8 * (L + p + 1), D->knots);
+  M.obs_kind = (const int*)alloc(4 * (size_t)D->n_obs, D->obs_kind);
+  M.obs_off = (const int*)alloc(16 * (size_t)D->n_obs, D->obs_off);
+  M.shift_desc = (const int*)alloc(4 * sd.size(), sd.data());
+  M.shift_T = (const double*)alloc(d8 * nT, D->shift_T);
+  M.x_tpl = (const double*)alloc(d8 * n, D->x_template);
+  M.p_tpl = (const double*)alloc(d8 * np_, D->p_template);
+  M.X = (double*)alloc(d8 * b * n, nullptr);
+  M.X0 = (double*)alloc(d8 * b * n, nullptr);
+  M.Xn = (double*)alloc(d8 * b * n, nullptr);
+  M.P = (double*)alloc(d8 * b * np_, nullptr);
+  M.t = (double*)alloc(d8 * b, nullptr);
+  M.t_prev = (double*)alloc(d8 * b, nullptr);
+  M.pred_x = (double*)alloc(d8 * b * nd, nullptr);
+  M.pred_u = (double*)alloc(d8 * b * nd, nullptr);
+  M.U = (double*)alloc(d8 * b * (n_samp + 1) * nd, nullptr);
+  M.rec = (int*)alloc(4 * b, nullptr);
+  q->lam = (double*)alloc(d8 * b * h->T.m, nullptr);
+  q->f = (double*)alloc(d8 * b, nullptr);
+  q->mask = (int*)alloc(4 * b, nullptr);
+  q->s0 = (double*)alloc(d8 * b * nd, nullptr);
+  q->sT = (double*)alloc(d8 * b * nd, nullptr);
+  q->obs = (double*)alloc(d8 * b * D->n_obs * (3 * nd + 1), nullptr);
+  q->xtraj = (double*)alloc(d8 * b * traj_len * nd, nullptr);
+  q->utraj = (double*)alloc(d8 * b * traj_len * nd, nullptr);
+  q->st = (int*)alloc(4 * b, nullptr);
+  q->it = (int*)alloc(4 * b, nullptr);
+  q->smem_prepare = 2 * d8 * n;
+  q->smem_commit = 2 * d8 * nd * L;
+  if (ok && q->smem_prepare > 48 * 1024 &&
+      cudaFuncSetAttribute((const void*)omg_mpc_prepare_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                           (int)q->smem_prepare) != cudaSuccess) ok = false;
+  if (!ok) { set_err("omg_mpc_create: device allocation/upload failed"); omg_mpc_destroy(q); return nullptr; }
+  return q;
+}
+
+int omg_mpc_update(omg_mpc* q, const double* state0, const double* stateT, const double* obstacles,
+                   double* state_traj, double* input_traj, int32_t* status, int32_t* iters, void* stream_) {
+  if (!q || !state0 || !stateT || (q && q->M.n_obs > 0 && !obstacles) || !state_traj || !input_traj || !status ||
+      !iters) { set_err("omg_mpc_update: null argument"); return -1; }
+  cudaStream_t stream = (cudaStream_t)stream_;
+  omg_problem* h = q->h;
+  CK(cudaSetDevice(h->device));
+  const int B = q->M.B;
+  OMG_LAUNCH(omg_mpc_prepare_kernel, B, OMG_MPC_NT, q->smem_prepare, stream, q->M, state0, stateT, obstacles);
+  CK(cudaGetLastError());
+  if (omg_solve_batch(h, B, q->M.X0, q->M.P, h->lbg, h->ubg, 1, nullptr, q->M.Xn, q->lam, q->f, status, iters, stream))
+    return -1;
+  OMG_LAUNCH(omg_mpc_commit_kernel, B, OMG_MPC_NT, q->smem_commit, stream, q->M, status, state_traj, input_traj);
+  CK(cudaGetLastError());
+  return 0;
+}
+
+int omg_mpc_update_host(omg_mpc* q, const double* state0, const double* stateT, const double* obstacles,
+                        double* state_traj, double* input_traj, int32_t* status, int32_t* iters) {
+  if (!q || !state0 || !stateT || (q && q->M.n_obs > 0 && !obstacles) || !state_traj || !input_traj || !status ||
+      !iters) { set_err("omg_mpc_update_host: null argument"); return -1; }
+  CK(cudaSetDevice(q->h->device));
+  const size_t b = q->M.B, nd = q->M.nd, no = (size_t)q->M.n_obs * (3 * nd + 1), nt = (size_t)q->M.traj_len * nd;
+  CK(cudaMemcpy(q->s0, state0, b * nd * 8, cudaMemcpyHostToDevice));
+  CK(cudaMemcpy(q->sT, stateT, b * nd * 8, cudaMemcpyHostToDevice));
+  if (no) CK(cudaMemcpy(q->obs, obstacles, b * no * 8, cudaMemcpyHostToDevice));
+  // (the rows of a failed solve keep what the caller's buffers hold)
+  CK(cudaMemcpy(q->xtraj, state_traj, b * nt * 8, cudaMemcpyHostToDevice));
+  CK(cudaMemcpy(q->utraj, input_traj, b * nt * 8, cudaMemcpyHostToDevice));
+  if (omg_mpc_update(q, q->s0, q->sT, q->obs, q->xtraj, q->utraj, q->st, q->it, nullptr)) return -1;
+  CK(cudaMemcpy(state_traj, q->xtraj, b * nt * 8, cudaMemcpyDeviceToHost));
+  CK(cudaMemcpy(input_traj, q->utraj, b * nt * 8, cudaMemcpyDeviceToHost));
+  CK(cudaMemcpy(status, q->st, b * 4, cudaMemcpyDeviceToHost));
+  CK(cudaMemcpy(iters, q->it, b * 4, cudaMemcpyDeviceToHost));
+  return 0;
+}
+
+int omg_mpc_recover(omg_mpc* q, const int32_t* mask) {
+  if (!q || !mask) { set_err("omg_mpc_recover: null argument"); return -1; }
+  CK(cudaSetDevice(q->h->device));
+  CK(cudaMemcpy(q->mask, mask, (size_t)q->M.B * 4, cudaMemcpyHostToDevice));
+  OMG_LAUNCH(omg_mpc_flag_kernel, (q->M.B + 127) / 128, 128, 0, nullptr, q->M.B, q->mask, q->M.rec);
+  CK(cudaGetLastError());
+  CK(cudaStreamSynchronize(nullptr));
+  return 0;
+}
+
+int omg_mpc_time(omg_mpc* q, double* t_out) {
+  if (!q || !t_out) { set_err("omg_mpc_time: null argument"); return -1; }
+  CK(cudaSetDevice(q->h->device));
+  CK(cudaDeviceSynchronize());
+  CK(cudaMemcpy(t_out, q->M.t, (size_t)q->M.B * 8, cudaMemcpyDeviceToHost));
+  return 0;
+}
+
+int omg_mpc_last_problem(omg_mpc* q, double* x0_out, double* p_out, void* stream_) {
+  if (!q) { set_err("omg_mpc_last_problem: null argument"); return -1; }
+  cudaStream_t stream = (cudaStream_t)stream_;
+  CK(cudaSetDevice(q->h->device));
+  const size_t b = q->M.B;
+  if (x0_out) CK(cudaMemcpyAsync(x0_out, q->M.X0, b * q->M.n * 8, cudaMemcpyDeviceToDevice, stream));
+  if (p_out) CK(cudaMemcpyAsync(p_out, q->M.P, b * q->M.n_par * 8, cudaMemcpyDeviceToDevice, stream));
   return 0;
 }
 

@@ -79,6 +79,22 @@ class _Options(C.Structure):
                 ('inertia_mode', C.c_int32), ('reserved', C.c_int32)]
 
 
+# include/omg_b200.h omg_mpc_desc: (name, kind), kind 'i' int32, 'd' float64, 'I' int32 array,
+# 'D' float64 array; the records of an MPC file carry the same names
+MPC_FIELDS = [('n', 'i'), ('n_par', 'i'), ('n_dim', 'i'), ('spl_offset', 'i'), ('L', 'i'), ('degree', 'i'),
+              ('knots', 'D'), ('horizon', 'd'), ('knot_time', 'd'), ('update_time', 'd'), ('sample_time', 'd'),
+              ('p_state0', 'i'), ('p_input0', 'i'), ('p_poseT', 'i'), ('p_t', 'i'), ('p_T', 'i'),
+              ('n_obs', 'i'), ('obs_kind', 'I'), ('obs_off', 'I'), ('n_shift', 'i'), ('shift_off', 'I'),
+              ('shift_len', 'I'), ('shift_ncol', 'I'), ('shift_T', 'D'), ('x_template', 'D'), ('p_template', 'D')]
+_CTYPE = {'i': C.c_int32, 'd': C.c_double, 'I': _i32p, 'D': _f64p}
+
+
+class _MpcDesc(C.Structure):
+    _fields_ = [(name, _CTYPE[kind]) for name, kind in MPC_FIELDS]
+
+
+MPC_PREDICTION = {'ideal': 0, 'integrate': 1}
+
 EXPORTS = ['omg_abi_version', 'omg_last_error', 'omg_default_options',
            'omg_problem_create', 'omg_problem_destroy', 'omg_set_options',
            'omg_solve_batch', 'omg_solve_batch_host', 'omg_shift_batch',
@@ -87,7 +103,9 @@ EXPORTS = ['omg_abi_version', 'omg_last_error', 'omg_default_options',
            'omg_tables_free', 'omg_integrate_rk4', 'omg_feas_batch', 'omg_feas_batch_host',
            'omg_comm_unique_id', 'omg_comm_create', 'omg_comm_destroy', 'omg_admm_exchange_x',
            'omg_admm_zl_update_dist', 'omg_closed_loop_step', 'omg_closed_loop_step_der',
-           'omg_shift_free_batch', 'omg_eval_batch', 'omg_closed_loop_step_free', 'omg_closed_loop_step_fleet']
+           'omg_shift_free_batch', 'omg_eval_batch', 'omg_closed_loop_step_free', 'omg_closed_loop_step_fleet',
+           'omg_mpc_read', 'omg_mpc_free_desc', 'omg_mpc_create', 'omg_mpc_destroy', 'omg_mpc_update',
+           'omg_mpc_update_host', 'omg_mpc_recover', 'omg_mpc_time', 'omg_mpc_last_problem']
 
 _lib = None
 
@@ -158,6 +176,19 @@ def bind(lib):
     lib.omg_shift_free_batch.argtypes = [vp, C.c_int32, vp, C.c_int32, C.c_double, vp, C.c_int32] + [vp] * 6
     lib.omg_eval_batch.argtypes = [C.c_int32, C.c_int32, vp, C.c_int32] + [vp] * 5 + [C.c_int32, vp, vp, C.c_int32,
                                                                                     vp, vp]
+    lib.omg_mpc_read.argtypes = [C.c_char_p]
+    lib.omg_mpc_read.restype = C.POINTER(_MpcDesc)
+    lib.omg_mpc_free_desc.argtypes = [C.POINTER(_MpcDesc)]
+    lib.omg_mpc_free_desc.restype = None
+    lib.omg_mpc_create.argtypes = [vp, C.POINTER(_MpcDesc), C.c_int32, C.c_int32, C.c_int32]
+    lib.omg_mpc_create.restype = C.c_void_p
+    lib.omg_mpc_destroy.argtypes = [vp]
+    lib.omg_mpc_destroy.restype = None
+    lib.omg_mpc_update.argtypes = [vp] * 9
+    lib.omg_mpc_update_host.argtypes = [vp] * 8
+    lib.omg_mpc_recover.argtypes = [vp, vp]
+    lib.omg_mpc_time.argtypes = [vp, vp]
+    lib.omg_mpc_last_problem.argtypes = [vp] * 4
     lib.omg_tables_read.argtypes = [C.c_char_p]
     lib.omg_tables_read.restype = C.POINTER(_Tables)
     lib.omg_tables_free.argtypes = [C.POINTER(_Tables)]
@@ -342,6 +373,82 @@ def save_tables(tb, path):
             if len(nb) > 23:
                 raise ValueError('record name too long: %s' % name)
             fp.write(nb.ljust(24, b'\0'))
+            fp.write(struct.pack('<iiq', dtype, 0, a.size))
+            fp.write(a.tobytes())
+
+
+def mpc_desc(problem, update_time=0.1, sample_time=0.01):
+    """The descriptor of the device-resident MPC update (include/omg_b200.h, omg_mpc_desc) of a
+    fixed-horizon Point2point with one Holonomic or Holonomic3D vehicle, as a dict of the
+    MPC_FIELDS.  Raises NotImplementedError naming the cause for anything else."""
+    from ..problems.point2point import FreeTPoint2point
+    if isinstance(problem, FreeTPoint2point):
+        raise NotImplementedError('the device MPC update has a fixed horizon only, not a free motion time '
+                                  '(FreeTPoint2point)')
+    if len(problem.vehicles) != 1:
+        raise NotImplementedError('the device MPC update runs one vehicle, this problem has %d'
+                                  % len(problem.vehicles))
+    veh = problem.vehicles[0]
+    if type(veh).__name__ not in ('Holonomic', 'Holonomic3D'):
+        raise NotImplementedError('the device MPC update runs a Holonomic or Holonomic3D vehicle, not %s'
+                                  % type(veh).__name__)
+    nd = veh.n_dim
+    for o in problem.environment.obstacles:
+        if o.options.get('spline_traj'):
+            raise NotImplementedError('the device MPC update takes obstacles that move with x/v/a or rotate, '
+                                      'not %s with a spline trajectory (spline_traj)' % o.label)
+        if o.n_dim != nd:
+            raise NotImplementedError('obstacle %s has %d dimensions, the vehicle %d' % (o.label, o.n_dim, nd))
+    father = problem.father
+    par = father._par_struct.entries
+    var = father._var_struct.entries
+    kind, off = [], []
+    for o in problem.environment.obstacles:
+        rot = (o.label, 'theta') in par
+        kind.append(int(rot))
+        off.append([par[(o.label, k)][0] for k in ('x', 'v', 'a')] + [par[(o.label, 'theta')][0] if rot else -1])
+    shifted = father.shifted_entries()
+    lab, basis = problem.label, veh.basis
+    return {
+        'n': father.tables.n, 'n_par': father.tables.n_par, 'n_dim': nd,
+        'spl_offset': var[(veh.label, 'splines_seg0')][0], 'L': len(basis), 'degree': basis.degree,
+        'knots': np.asarray(basis.knots, dtype=np.float64),
+        'horizon': float(problem.options['horizon_time']), 'knot_time': float(problem.knot_time),
+        'update_time': float(update_time), 'sample_time': float(sample_time),
+        'p_state0': par[(veh.label, 'state0')][0], 'p_input0': par[(veh.label, 'input0')][0],
+        'p_poseT': par[(veh.label, 'poseT')][0], 'p_t': par[(lab, 't')][0], 'p_T': par[(lab, 'T')][0],
+        'n_obs': len(kind), 'obs_kind': np.array(kind, dtype=np.int32),
+        'obs_off': np.array(off, dtype=np.int32).reshape(-1),
+        'n_shift': len(shifted), 'shift_off': np.array([e[2] for e in shifted], dtype=np.int32),
+        'shift_len': np.array([e[3][0] for e in shifted], dtype=np.int32),
+        'shift_ncol': np.array([e[3][1] for e in shifted], dtype=np.int32),
+        'shift_T': np.concatenate([np.asarray(e[4], dtype=np.float64).reshape(-1) for e in shifted] + [np.zeros(0)]),
+        'x_template': np.asarray(father.get_variables().cat, dtype=np.float64),
+        'p_template': np.asarray(father.set_parameters(0.).cat, dtype=np.float64)}
+
+
+def pack_mpc_desc(desc):
+    """mpc_desc dict -> (ctypes omg_mpc_desc, keep-alive object)."""
+    keep, D = _Keep(), _MpcDesc()
+    for name, kind in MPC_FIELDS:
+        v = desc[name]
+        cast = {'i': int, 'd': float, 'I': keep.i32, 'D': keep.f64}[kind]
+        setattr(D, name, cast(v))
+    return D, keep
+
+
+def save_mpc(problem, path, update_time=0.1, sample_time=0.01):
+    """Write the descriptor of the device MPC update to an MPC file (include/omg_b200.h:
+    omg_mpc_read), the companion of save_tables for native callers of omg_mpc_update."""
+    import struct
+    desc = mpc_desc(problem, update_time, sample_time)
+    with open(path, 'wb') as fp:
+        fp.write(b'OMGMPC\0\0')
+        fp.write(struct.pack('<ii', ABI_VERSION, len(MPC_FIELDS)))
+        for name, kind in MPC_FIELDS:
+            dtype = 1 if kind in 'dD' else 0
+            a = np.ascontiguousarray(desc[name], dtype=np.float64 if dtype else np.int32).reshape(-1)
+            fp.write(name.encode().ljust(24, b'\0'))
             fp.write(struct.pack('<iiq', dtype, 0, a.size))
             fp.write(a.tobytes())
 
