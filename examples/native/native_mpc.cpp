@@ -1,7 +1,8 @@
 // Native receding-horizon loop on libomgb200.so: the C++ twin of a deployed controller calling the
 // reference's exported Point2Point::update() (omgtools/export/point2point/Point2Point.cpp:119-205)
 // for B independent instances at once.  The deployable artefacts are a table file
-// (omg_tools_b200.solver.b200.save_tables) and an MPC file (save_mpc); no Python and no CasADi at
+// (omg_tools_b200.solver.b200.save_tables) and an MPC file (save_mpc for a fixed horizon,
+// save_mpc_freeT for a free motion time; the example reads either); no Python and no CasADi at
 // run time.
 //
 //   g++ -O2 -I include examples/native/native_mpc.cpp -o native_mpc \
@@ -38,11 +39,14 @@ int main(int argc, char** argv) {
   }
   omg_tables* tb = omg_tables_read(argv[1]);
   if (!tb) { fprintf(stderr, "tables: %s\n", omg_last_error()); return 1; }
+  // a fixed-horizon MPC file, else a free-T one
   omg_mpc_desc* desc = omg_mpc_read(argv[2]);
-  if (!desc) { fprintf(stderr, "mpc: %s\n", omg_last_error()); return 1; }
-  const int B = atoi(argv[3]), N = atoi(argv[4]), tl = atoi(argv[5]), nd = desc->n_dim;
+  omg_mpc_freeT_desc* fdesc = desc ? nullptr : omg_mpc_freet_read(argv[2]);
+  if (!desc && !fdesc) { fprintf(stderr, "mpc: %s\n", omg_last_error()); return 1; }
+  const int B = atoi(argv[3]), N = atoi(argv[4]), tl = atoi(argv[5]);
+  const int nd = desc ? desc->n_dim : fdesc->n_dim, n_obs = desc ? desc->n_obs : fdesc->n_obs;
   const int mode = strcmp(argv[6], "integrate") == 0 ? OMG_MPC_PREDICT_INTEGRATE : OMG_MPC_PREDICT_IDEAL;
-  std::vector<double> state0((size_t)B * nd), stateT((size_t)B * nd), obs((size_t)B * desc->n_obs * (3 * nd + 1));
+  std::vector<double> state0((size_t)B * nd), stateT((size_t)B * nd), obs((size_t)B * n_obs * (3 * nd + 1));
   if (!read_doubles(argv[7], state0) || !read_doubles(argv[8], stateT) || !read_doubles(argv[9], obs)) {
     fprintf(stderr, "bad input files\n"); return 1;
   }
@@ -50,7 +54,7 @@ int main(int argc, char** argv) {
   omg_default_options(&opt);
   omg_problem* h = omg_problem_create(tb, &opt, 0);
   if (!h) { fprintf(stderr, "create: %s\n", omg_last_error()); return 1; }
-  omg_mpc* mpc = omg_mpc_create(h, desc, B, tl, mode);
+  omg_mpc* mpc = desc ? omg_mpc_create(h, desc, B, tl, mode) : omg_mpc_create_freet(h, fdesc, B, tl, mode);
   if (!mpc) { fprintf(stderr, "mpc create: %s\n", omg_last_error()); return 1; }
   std::vector<double> xtraj((size_t)B * tl * nd, 0.0), utraj((size_t)B * tl * nd, 0.0);
   std::vector<int32_t> status(B), iters(B);
@@ -63,7 +67,8 @@ int main(int argc, char** argv) {
     }
     for (int b = 0; b < B; ++b) {
       printf("update %d instance %d status %d iters %d\n", k, b, status[b], iters[b]);
-      // a failed instance keeps its state: Point2Point::update returned false, the caller may recover
+      // a failed instance keeps its state: Point2Point::update returned false, the caller may recover;
+      // a stopped one (free motion time, OMG_MPC_STOPPED) has arrived
       if (status[b] == OMG_SOLVE_SUCCEEDED)
         for (int c = 0; c < nd; ++c) state0[(size_t)b * nd + c] = xtraj[(size_t)b * tl * nd + c];
     }
@@ -74,6 +79,7 @@ int main(int argc, char** argv) {
   omg_mpc_destroy(mpc);
   omg_problem_destroy(h);
   omg_mpc_free_desc(desc);
+  omg_mpc_freet_release(fdesc);
   omg_tables_free(tb);
   return 0;
 }

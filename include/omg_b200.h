@@ -180,6 +180,17 @@ int omg_solve_batch(omg_problem* h, int32_t B,
                     double* x, double* lam_g, double* f,
                     int32_t* status, int32_t* iters, void* stream);
 
+/* omg_solve_batch on the rows listed in DEVICE rows [*n_rows] (n_rows a DEVICE int32): listed
+ * entry i solves row rows[i] of every buffer; an unlisted row's outputs are not written.  The
+ * launch shape depends on B only, so the list may change between replays of a CUDA graph. */
+int omg_solve_batch_rows(omg_problem* h, int32_t B,
+                         const double* x0, const double* p,
+                         const double* lbg, const double* ubg, int32_t bounds_shared,
+                         const double* lam_g0,
+                         double* x, double* lam_g, double* f,
+                         int32_t* status, int32_t* iters,
+                         const int32_t* rows, const int32_t* n_rows, void* stream);
+
 /* Same call with HOST buffers: H2D of inputs, solve, D2H of results,
  * synchronous.  This is the call the reference-facing plugin times end to end. */
 int omg_solve_batch_host(omg_problem* h, int32_t B,
@@ -520,7 +531,8 @@ void omg_tables_free(omg_tables* tables);
  *            (Point2Point::update returns false).  status[b] and iters[b] are always written.
  * Obstacles are supplied on every call in their current state (the reference's obstacle_t):
  * obstacles[b] holds n_obs records of 3 * n_dim + 1 doubles, {x, v, a, theta}; theta is read only
- * for a rotating obstacle.  Not covered: a free horizon, several vehicles, other vehicles, run-time
+ * for a rotating obstacle.  A free motion time (FreeTPoint2point) has its own descriptor and create
+ * call below and shares every other call.  Not covered: several vehicles, other vehicles, run-time
  * bounds (updateBounds), predict_shift and provide_prediction. */
 typedef struct omg_mpc omg_mpc;   /* opaque handle */
 
@@ -573,6 +585,77 @@ int omg_mpc_update_host(omg_mpc* mpc, const double* state0, const double* stateT
 /* Cold-start the instances with mask[b] != 0 (HOST int32 [B]) on their next update, as
  * Point2Point::recover().  Synchronous: the flags are set when the call returns. */
 int omg_mpc_recover(omg_mpc* mpc, const int32_t* mask);
+/* ---- free motion time (FreeTPoint2point): T is a decision variable ----------------------------
+ * The same handle type, created by omg_mpc_create_freet; omg_mpc_update(_host), omg_mpc_recover,
+ * omg_mpc_time, omg_mpc_motion_time, omg_mpc_last_problem and omg_mpc_destroy serve both kinds.
+ * Per instance b, with T_b the motion time of its last accepted plan (x[t_index]), dt =
+ * update_time, st = sample_time and round6 as above:
+ *   prepare  cold start on the first update and after omg_mpc_recover (a stopped instance
+ *            included): x_template with linspace(state0, stateT, L) in the vehicle's columns
+ *            and the template's T, state0 = the caller's state0[b], input0 = 0.
+ *            After an accepted solve: the prediction from that plan on its own time axis
+ *            (ideal: value and derivative / T_b at min(dt, T_b) / T_b; integrate: classical RK4
+ *            from the caller's state0[b] over the planned inputs at s st / T_b, s = 0 ..
+ *            round6(min(dt, T_b) / st), linearly interpolated, input0 = the last of them), then
+ *            the stop test: the instance stops when T_b < dt, or when |state0 - stateT[b]| <=
+ *            stop_tol and |input0| <= stop_tol (holonomic.py check_terminal_conditions).  A
+ *            running instance is shifted from its plan's T (FreeTPoint2point.init_step):
+ *            u, target = (dt, T_b - dt), or (T_b - dt, T_b) when T_b < 2 dt; tau = u / target;
+ *            every block is re-expressed on shift_spline's basis (omg_shift_free_batch's
+ *            arithmetic) when 0 < tau < 1, and x[t_index] = target.
+ *            After a failed solve: no shift, the same warm start and stored prediction.
+ *            P[b] is p_template with state0, input0, poseT = stateT[b] and the obstacles written
+ *            in (t stays 0; there is no T parameter).
+ *   solve    omg_solve_batch_rows on the instances that are not stopped.
+ *   commit   a stopped instance: status OMG_MPC_STOPPED, 0 iterations; its time, warm start,
+ *            motion time and output rows stay as they are until omg_mpc_recover.  Status 0: the
+ *            x row takes the solution, state_traj[b] / input_traj[b] row j are the plan's value
+ *            and derivative / T at min(j st, T) / T (rows past the plan hold its final point),
+ *            the next prediction's samples are stored and t_b = round6(t_b + dt).  Any other
+ *            status: as with a fixed horizon (the warm start, time and output rows are kept).
+ * After the first update an update makes no synchronous call and no allocation, so updates stay
+ * capturable in a CUDA graph, across the updates at which instances stop too. */
+enum { OMG_MPC_STOPPED = -1 };    /* status of an instance not solved because it has stopped */
+
+typedef struct omg_mpc_freeT_desc {
+  int32_t n, n_par;               /* the problem's sizes */
+  int32_t n_dim;                  /* vehicle: states = inputs = position splines, 1 .. 3 */
+  int32_t spl_offset;             /* column c of the vehicle's splines at x[spl_offset + c * L] */
+  int32_t L, degree;              /* the vehicle's B-spline basis on [0, 1] */
+  const double* knots;            /* [L + degree + 1] */
+  double update_time, sample_time;
+  double stop_tol;                /* the vehicle's stop_tol */
+  int32_t t_index;                /* offset of the motion time T in x */
+  int32_t p_state0, p_input0, p_poseT;   /* offsets in p */
+  int32_t n_obs;
+  const int32_t* obs_kind;        /* [n_obs] as in omg_mpc_desc */
+  const int32_t* obs_off;         /* [n_obs * 4] */
+  int32_t n_blocks;               /* the spline blocks the warm start re-expresses */
+  const int32_t* blk_off;         /* [n_blocks] offset in x */
+  const int32_t* blk_len;         /* [n_blocks] basis length L */
+  const int32_t* blk_ncol;        /* [n_blocks] columns */
+  const int32_t* blk_degree;      /* [n_blocks] degree p */
+  const double* blk_knots;        /* the n_blocks knot vectors [L + p + 1], concatenated */
+  const double* x_template;       /* [n] father.get_variables().cat (holds the initial T) */
+  const double* p_template;       /* [n_par] father.set_parameters(0.).cat */
+} omg_mpc_freeT_desc;
+
+/* MPC files of the free-T descriptor: the container of omg_mpc_read with records named after the
+ * fields of omg_mpc_freeT_desc (written by omg_tools_b200.solver.b200.save_mpc_freeT).  Each
+ * reader refuses the other kind's file, naming the other reader. */
+omg_mpc_freeT_desc* omg_mpc_freet_read(const char* path);
+void omg_mpc_freet_release(omg_mpc_freeT_desc* desc);
+
+/* Returns NULL with a message for what omg_mpc_create rejects (but the horizon and knot time),
+ * t_index outside x, a block outside x or beyond OMG_SPL_MAX_DEGREE / OMG_SPL_MAX_LEN, knots that
+ * decrease, stop_tol < 0 and trajectory_length outside 1 .. (template T) / sample_time. */
+omg_mpc* omg_mpc_create_freet(omg_problem* problem, const omg_mpc_freeT_desc* desc, int32_t B,
+                              int32_t trajectory_length, int32_t prediction);
+
+/* Each instance's T of its last accepted plan (the template's before the first) into DEVICE
+ * T_out [B]; the horizon for a fixed-horizon handle.  Asynchronous on `stream`. */
+int omg_mpc_motion_time(omg_mpc* mpc, double* T_out, void* stream);
+
 /* Current time t_b of every instance into HOST t_out [B] (synchronises the device). */
 int omg_mpc_time(omg_mpc* mpc, double* t_out);
 /* The warm start and parameter rows handed to the last solve, DEVICE x0_out [B][n] and p_out

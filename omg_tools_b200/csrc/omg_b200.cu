@@ -110,7 +110,17 @@ struct Batch {
   double *x, *lam, *f; int *status, *iters;
   double* dscr; int* iscr; int dscr_stride, iscr_stride;
   int* counter; double* trace;
+  // optional row list: instance i of the counter is row rows[i], for i < *n_rows (both null: row i
+  // for i < B).  Rows index x0, p, the bounds and every output.
+  const int* rows; const int* n_rows;
 };
+
+// The row the persistent grid takes next (thread 0 of a block); B when none is left.
+__device__ __forceinline__ int omg_next_row(const Batch& A) {
+  const int i = atomicAdd(A.counter, 1);
+  if (!A.rows) return i;
+  return i < *A.n_rows ? A.rows[i] : A.B;
+}
 
 struct Ctl {                       // uniform per-block control scalars
   double mu, tau, theta_max, theta_min, delta_w, delta_w_last, delta_c;
@@ -544,7 +554,7 @@ __device__ __forceinline__ void ipm_body(const DevTab& T, const omg_options& O, 
 
   for (;;) {
     // ---- fetch next instance ------------------------------------------------
-    if (tid == 0) ctl.inst = atomicAdd(A.counter, 1);
+    if (tid == 0) ctl.inst = omg_next_row(A);
     __syncthreads();
     const int inst = ctl.inst;
     if (inst >= A.B) return;
@@ -1612,36 +1622,34 @@ __device__ __forceinline__ double omg_linspace(double a, double b, int num, int 
   return i == num - 1 ? b : __dadd_rn(__dmul_rn((double)i, (b - a) / (double)(num - 1)), a);
 }
 
-// Free-T warm start of one instance per block (reference FreeTPoint2point.init_step,
-// point2point.py:354-368, with shift_spline, spline_extra.py:88-99): from T = x[t_index] the
-// update u and target time (u = T - dt, target = T when T < 2 dt; else u = dt, target = T - dt),
-// tau = u / target; every block is re-expressed on shift_spline's basis
+// The update u and target time of a free-T warm start from the motion time T (reference
+// FreeTPoint2point.init_step, point2point.py:354-368): u = T - dt, target = T when T < 2 dt; else
+// u = dt, target = T - dt.  Returns tau = u / target.
+__device__ __forceinline__ double omg_free_shift_tau(double T, double dt, double* target) {
+  double u = dt;
+  *target = T - dt;
+  if (T < 2.0 * dt) { u = T - dt; *target = T; }
+  return u / *target;
+}
+
+// Free-T re-expression of one x row by the threads of a block (shift_spline, spline_extra.py:88-99):
+// every block is re-expressed on shift_spline's basis
 //   knots2 = [tau] * p + linspace(tau, end, L - p + 1) + [end] * p
 // by BSplineBasis.transform: collocation at the first arg-max of each new basis function over
 // linspace(tau, end, 501), M = bm^-1 old_basis(points), entries below 1e-10 dropped, c <- M c.
-// Then x[t_index] = target.  Inactive instances and tau outside (0, 1) are left alone.
-// Shared memory: x row [n] | knots2 [Lmax + pmax + 1] | points [Lmax] | arg-max scratch
-// [2 blockDim] | bm [Lmax^2] | old_basis(points), then M [Lmax^2].
-__global__ void omg_shift_free_kernel(double* x, int B, int n, int t_index, double dt,
-                                      const int* __restrict__ active, int n_blocks,
-                                      const int* __restrict__ desc, const double* __restrict__ kn,
-                                      int Lmax, int pmax) {
-  OMG_DYN_SHARED(xs);
-  const int b = blockIdx.x, t = threadIdx.x, nt = blockDim.x;
-  if (b >= B || (active && !active[b])) return;
-  double* xb = x + (size_t)b * n;
-  const double T = xb[t_index];
-  double u = dt, target = T - dt;
-  if (T < 2.0 * dt) { u = T - dt; target = T; }
-  const double tau = u / target;
-  if (!(tau > 0.0 && tau < 1.0)) return;
-  double* k2 = xs + n;
+// xs: the source row in shared memory, loaded by the caller (the first barrier below orders it);
+// xb: the destination row (must not alias xs).  sm: shared scratch of knots2 [Lmax + pmax + 1] |
+// points [Lmax] | arg-max scratch [2 blockDim] | bm [Lmax^2] | old_basis(points), then M [Lmax^2].
+__device__ __forceinline__ void omg_shift_free_row(const double* xs, double* xb, double tau, int n_blocks,
+                                                   const int* __restrict__ desc, const double* __restrict__ kn,
+                                                   int Lmax, int pmax, double* sm) {
+  const int t = threadIdx.x, nt = blockDim.x;
+  double* k2 = sm;
   double* xm = k2 + Lmax + pmax + 1;
   double* sv = xm + Lmax;
   double* sg = sv + nt;
   double* A = sg + nt;
   double* R = A + (size_t)Lmax * Lmax;
-  for (int i = t; i < n; i += nt) xs[i] = xb[i];
   for (int blk = 0; blk < n_blocks; ++blk) {
     const int* dsc = desc + OMG_SPL_DESC * blk;
     const int off = dsc[0], L = dsc[1], nc = dsc[2], p = dsc[3];
@@ -1717,6 +1725,25 @@ __global__ void omg_shift_free_kernel(double* x, int B, int n, int t_index, doub
       xb[off + c * L + i] = acc;
     }
   }
+}
+
+// Free-T warm start of one instance per block (reference FreeTPoint2point.init_step with
+// shift_spline): tau from T = x[t_index] (omg_free_shift_tau), the row re-expressed in place
+// (omg_shift_free_row), then x[t_index] = target.  Inactive instances and tau outside (0, 1) are
+// left alone.  Shared memory: x row [n] | the scratch of omg_shift_free_row.
+__global__ void omg_shift_free_kernel(double* x, int B, int n, int t_index, double dt,
+                                      const int* __restrict__ active, int n_blocks,
+                                      const int* __restrict__ desc, const double* __restrict__ kn,
+                                      int Lmax, int pmax) {
+  OMG_DYN_SHARED(xs);
+  const int b = blockIdx.x, t = threadIdx.x, nt = blockDim.x;
+  if (b >= B || (active && !active[b])) return;
+  double* xb = x + (size_t)b * n;
+  double target;
+  const double tau = omg_free_shift_tau(xb[t_index], dt, &target);
+  if (!(tau > 0.0 && tau < 1.0)) return;
+  for (int i = t; i < n; i += nt) xs[i] = xb[i];
+  omg_shift_free_row(xs, xb, tau, n_blocks, desc, kn, Lmax, pmax, xs + n);
   __syncthreads();                                // (every thread has read T)
   if (t == 0) xb[t_index] = target;
 }
@@ -2636,10 +2663,16 @@ int omg_get_info(omg_problem* h, int32_t* n, int32_t* m, int32_t* n_par, int32_t
 const char* omg_structure_info(omg_problem* h) { return h ? h->sp_info.c_str() : ""; }
 const char* omg_envelope_layout(omg_problem* h) { return h ? h->env_info.c_str() : ""; }
 
-int omg_solve_batch(omg_problem* h, int32_t B, const double* x0, const double* p,
-                    const double* lbg, const double* ubg, int32_t bounds_shared,
-                    const double* lam_g0, double* x, double* lam_g, double* f,
-                    int32_t* status, int32_t* iters, void* stream_) {
+}  // extern "C"
+
+// omg_solve_batch on the rows listed in DEVICE rows [*n_rows] (ascending; both null: every row).
+// The grid is min(B, resident blocks) whatever the list holds, so the launch shape does not
+// depend on device data; an unlisted row's outputs are not written.
+static int solve_batch_rows(omg_problem* h, int32_t B, const double* x0, const double* p,
+                            const double* lbg, const double* ubg, int32_t bounds_shared,
+                            const double* lam_g0, double* x, double* lam_g, double* f,
+                            int32_t* status, int32_t* iters, const int* rows, const int* n_rows,
+                            void* stream_) {
   if (!h) { set_err("null handle"); return -1; }
   if (B <= 0) return 0;
   if (!x0 || !p || !lbg || !ubg || !x || !lam_g || !f || !status || !iters) { set_err("null buffer"); return -1; }
@@ -2663,6 +2696,7 @@ int omg_solve_batch(omg_problem* h, int32_t B, const double* x0, const double* p
   A.x = x; A.lam = lam_g; A.f = f; A.status = status; A.iters = iters;
   A.dscr = h->dscr; A.iscr = h->iscr; A.dscr_stride = h->dscr_stride; A.iscr_stride = h->iscr_stride;
   A.counter = h->counter; A.trace = h->trace;
+  A.rows = rows; A.n_rows = n_rows;
   CK(cudaMemsetAsync(h->counter, 0, sizeof(int), stream));
   CK(cudaEventRecord(h->ev0, stream));
   if (use_sp) OMG_LAUNCH(omg_ipm_kernel_sp, grid, h->P.nt, h->sp_smem_bytes, stream, h->T, h->P, h->opt, A, h->SS);
@@ -2680,6 +2714,26 @@ int omg_solve_batch(omg_problem* h, int32_t B, const double* x0, const double* p
   CK(cudaEventRecord(h->ev1, stream));
   h->timed = true; h->launches = 1;
   return 0;
+}
+
+extern "C" {
+
+int omg_solve_batch(omg_problem* h, int32_t B, const double* x0, const double* p,
+                    const double* lbg, const double* ubg, int32_t bounds_shared,
+                    const double* lam_g0, double* x, double* lam_g, double* f,
+                    int32_t* status, int32_t* iters, void* stream_) {
+  return solve_batch_rows(h, B, x0, p, lbg, ubg, bounds_shared, lam_g0, x, lam_g, f, status, iters, nullptr,
+                          nullptr, stream_);
+}
+
+int omg_solve_batch_rows(omg_problem* h, int32_t B, const double* x0, const double* p,
+                         const double* lbg, const double* ubg, int32_t bounds_shared,
+                         const double* lam_g0, double* x, double* lam_g, double* f,
+                         int32_t* status, int32_t* iters, const int32_t* rows, const int32_t* n_rows,
+                         void* stream_) {
+  if (!rows || !n_rows) { set_err("omg_solve_batch_rows: null row list"); return -1; }
+  return solve_batch_rows(h, B, x0, p, lbg, ubg, bounds_shared, lam_g0, x, lam_g, f, status, iters, rows, n_rows,
+                          stream_);
 }
 
 int omg_last_timing(omg_problem* h, float* kernel_ms, int32_t* launches) {
@@ -3337,7 +3391,20 @@ struct MpcDev {
   double* pred_u;           // [B][nd] and input
   double* U;                // [B][n_samp + 1][nd] integrate: planned inputs from t_rel
   int* rec;                 // [B] cold start requested by omg_mpc_recover
+  // free motion time (omg_mpc_create_freet)
+  int t_index, n_blocks, Lmax, pmax;
+  double stop_tol;
+  const int* blk_desc;      // [n_blocks][OMG_SPL_DESC] the shifted spline blocks (spline_desc)
+  const double* blk_knots;
+  double* Tm;               // [B] T of the last accepted plan
+  int* phase;               // [B] OMG_MPC_COLD / _ACCEPTED / _FAILED: what the last update left
+  int* stop;                // [B] stopped (not solved until omg_mpc_recover)
+  int* ns;                  // [B] integrate: the samples of U the next prediction spans
+  int* rows;                // [B] the rows solved by this update, ascending
+  int* n_rows;              // [1]
 };
+
+enum { OMG_MPC_COLD = 0, OMG_MPC_ACCEPTED = 1, OMG_MPC_FAILED = 2 };
 
 // numpy.round(x, 6)
 __device__ __forceinline__ double omg_round6(double x) { return rint(x * 1e6) / 1e6; }
@@ -3467,6 +3534,191 @@ __global__ void omg_mpc_commit_kernel(const MpcDev M, const int* __restrict__ st
   }
 }
 
+// Free motion time, shared memory: source x row [n] | warm start [n] | omg_shift_free_row's scratch.
+// Cold start: the template with linspace(state0, stateT) in the vehicle's columns.  After an accepted
+// solve: the prediction the commit stored (ideal) or RK4 from state0 over the stored inputs
+// (integrate), then the stop test on the accepted plan's T and that prediction; a running instance
+// is shifted from its plan's own T.  After a failed solve: the same warm start and prediction.  A
+// stopped instance writes nothing.
+__global__ void omg_mpc_prepare_free_kernel(const MpcDev M, const double* __restrict__ state0,
+                                            const double* __restrict__ stateT, const double* __restrict__ obs) {
+  OMG_DYN_SHARED(xs);
+  __shared__ int stop_s;
+  __shared__ double s0[OMG_ODE_MAX_STATE], u0[OMG_CL_MAX_INPUT];
+  const int b = blockIdx.x, t = threadIdx.x, nt = blockDim.x, n = M.n, nd = M.nd, L = M.L;
+  if (b >= M.B) return;
+  double* ws = xs + n;
+  const bool cold = M.rec[b] != 0 || M.phase[b] == OMG_MPC_COLD;
+  const bool accepted = !cold && M.phase[b] == OMG_MPC_ACCEPTED;
+  if (!cold && M.stop[b]) return;
+  const double* st0 = state0 + (size_t)b * nd;
+  const double* stT = stateT + (size_t)b * nd;
+  if (t == 0) {
+    if (cold) {                       // Holonomic::setInitialConditions
+      for (int c = 0; c < nd; ++c) { s0[c] = st0[c]; u0[c] = 0.0; }
+    } else if (M.mode == OMG_MPC_PREDICT_IDEAL) {
+      for (int c = 0; c < nd; ++c) { s0[c] = M.pred_x[(size_t)b * nd + c]; u0[c] = M.pred_u[(size_t)b * nd + c]; }
+    } else {                          // RK4 from the measured state over the planned inputs
+      const double* Ub = M.U + (size_t)b * (M.n_samp + 1) * nd;
+      const int ns = M.ns[b];
+      double y[OMG_ODE_MAX_STATE], st[OMG_ODE_MAX_STATE], k1[OMG_ODE_MAX_STATE], k2[OMG_ODE_MAX_STATE],
+             k3[OMG_ODE_MAX_STATE], k4[OMG_ODE_MAX_STATE], um[OMG_CL_MAX_INPUT];
+      for (int c = 0; c < nd; ++c) y[c] = st0[c];
+      omg_rk4_interp(OMG_ODE_INTEGRATOR, nd, nd, ns, M.sample_time, Ub, y, st, k1, k2, k3, k4, um);
+      for (int c = 0; c < nd; ++c) { s0[c] = y[c]; u0[c] = Ub[(size_t)ns * nd + c]; }
+    }
+    int stop = 0;
+    if (accepted) {                   // check_terminal_conditions (BatchMPC._at_goal), or T < update_time
+      double e2 = 0.0, u2 = 0.0;
+      for (int c = 0; c < nd; ++c) {
+        const double e = s0[c] - stT[c];
+        e2 = __dadd_rn(e2, __dmul_rn(e, e));
+        u2 = __dadd_rn(u2, __dmul_rn(u0[c], u0[c]));
+      }
+      stop = M.Tm[b] < M.update_time || (sqrt(e2) <= M.stop_tol && sqrt(u2) <= M.stop_tol);
+    }
+    stop_s = stop;
+  }
+  __syncthreads();                    // (every thread has read rec[b], phase[b] and stop[b])
+  if (t == 0) { M.stop[b] = stop_s; M.rec[b] = 0; }
+  if (stop_s) return;
+  const double* src = cold ? M.x_tpl : M.X + (size_t)b * n;
+  for (int i = t; i < n; i += nt) xs[i] = ws[i] = src[i];
+  __syncthreads();
+  if (cold) {                         // getInitSplineValue: linspace(state0, stateT, L) per column
+    for (int e = t; e < nd * L; e += nt) {
+      const int c = e / L, i = e - c * L;
+      ws[M.spl_off + e] = omg_linspace(st0[c], stT[c], L, i);
+    }
+  } else if (accepted) {              // FreeTPoint2point.init_step from the plan's own T
+    double target;
+    const double tau = omg_free_shift_tau(xs[M.t_index], M.update_time, &target);
+    if (tau > 0.0 && tau < 1.0) {
+      omg_shift_free_row(xs, ws, tau, M.n_blocks, M.blk_desc, M.blk_knots, M.Lmax, M.pmax, ws + n);
+      __syncthreads();
+      if (t == 0) ws[M.t_index] = target;
+    }
+  }
+  __syncthreads();
+  double* x0 = M.X0 + (size_t)b * n;
+  double* pb = M.P + (size_t)b * M.n_par;
+  for (int i = t; i < n; i += nt) x0[i] = ws[i];
+  for (int i = t; i < M.n_par; i += nt) pb[i] = M.p_tpl[i];
+  __syncthreads();                    // (the template row is in place)
+  if (t != 0) return;
+  for (int c = 0; c < nd; ++c) {
+    pb[M.p_state0 + c] = s0[c];
+    pb[M.p_input0 + c] = u0[c];
+    pb[M.p_poseT + c] = stT[c];
+  }
+  const int rl = 3 * nd + 1;
+  for (int k = 0; k < M.n_obs; ++k) {
+    const double* o = obs + ((size_t)b * M.n_obs + k) * rl;
+    const int* off = M.obs_off + 4 * k;
+    for (int c = 0; c < nd; ++c) {
+      pb[off[0] + c] = o[c];
+      pb[off[1] + c] = o[nd + c];
+      pb[off[2] + c] = o[2 * nd + c];
+    }
+    if (M.obs_kind[k]) pb[off[3]] = o[3 * nd];
+  }
+}
+
+// The rows that are not stopped, in ascending order, and their count: one block, a scan per chunk
+// of blockDim rows.  Shared memory: [blockDim] ints.
+__global__ void omg_mpc_rows_kernel(int B, const int* __restrict__ stop, int* __restrict__ rows, int* __restrict__ n_rows) {
+  OMG_DYN_SHARED(scd);
+  int* sc = reinterpret_cast<int*>(scd);
+  const int t = threadIdx.x, nt = blockDim.x;
+  int base = 0;
+  for (int c0 = 0; c0 < B; c0 += nt) {
+    const int live = (c0 + t < B && !stop[c0 + t]) ? 1 : 0;
+    sc[t] = live;
+    __syncthreads();
+    for (int d = 1; d < nt; d *= 2) {         // inclusive scan (Hillis-Steele)
+      const int v = t >= d ? sc[t - d] : 0;
+      __syncthreads();
+      sc[t] += v;
+      __syncthreads();
+    }
+    if (live) rows[base + sc[t] - 1] = c0 + t;
+    base += sc[nt - 1];
+    __syncthreads();
+  }
+  if (t == 0) *n_rows = base;
+}
+
+// Free motion time, shared memory as omg_mpc_commit_kernel.  A stopped instance reads nothing of the
+// solve: status -1, 0 iterations.  Status 0: the row takes the solution, the output rows are the
+// plan at min(j sample_time, T) / T, and the next prediction's samples are stored (ideal: at
+// min(update_time, T) / T; integrate: s sample_time / T for s <= round6(min(update_time, T) /
+// sample_time)).  Any other status keeps the warm start it was solved from.
+__global__ void omg_mpc_commit_free_kernel(const MpcDev M, int* __restrict__ status, int* __restrict__ iters,
+                                           double* __restrict__ state_traj, double* __restrict__ input_traj) {
+  OMG_DYN_SHARED(cd);
+  const int b = blockIdx.x, t = threadIdx.x, nt = blockDim.x, n = M.n, nd = M.nd, L = M.L, p = M.p;
+  if (b >= M.B) return;
+  if (M.stop[b]) {
+    if (t == 0) { status[b] = -1; iters[b] = 0; }
+    return;
+  }
+  const bool ok = status[b] == 0;
+  const double* src = (ok ? M.Xn : M.X0) + (size_t)b * n;
+  double* xb = M.X + (size_t)b * n;
+  for (int i = t; i < n; i += nt) xb[i] = src[i];
+  if (!ok) {                          // keep the warm start; a cold start stays one
+    if (t == 0 && M.phase[b] != OMG_MPC_COLD) M.phase[b] = OMG_MPC_FAILED;
+    return;
+  }
+  for (int c = t; c < nd; c += nt) omg_spl_der_coef(M.knots, p, L, 2, src + M.spl_off + c * L, cd + (size_t)c * 2 * L);
+  __syncthreads();
+  const double T = src[M.t_index], st = M.sample_time;
+  const bool ideal = M.mode == OMG_MPC_PREDICT_IDEAL;
+  const int ns = (int)omg_round6(fmin(M.update_time, T) / st);
+  const int tl = M.traj_len, n_pts = tl + (ideal ? 1 : ns + 1);
+  for (int j = t; j < n_pts; j += nt) {
+    const double tau = j < tl ? fmin((double)j * st, T) / T
+                       : ideal ? fmin(M.update_time, T) / T : (double)(j - tl) * st / T;
+    double w[OMG_SPL_MAX_LEN + OMG_SPL_MAX_DEGREE], v[2][OMG_CL_MAX_INPUT];
+    for (int d = 0; d < 2; ++d) {
+      omg_cox_de_boor(M.knots + d, p - d, tau, 0, L - d, w);
+      for (int c = 0; c < nd; ++c) {
+        const double* q = cd + ((size_t)c * 2 + d) * L;
+        double acc = 0.0;
+        for (int i = 0; i < L - d; ++i) acc += w[i] * q[i];
+        v[d][c] = d ? acc / T : acc;
+      }
+    }
+    double *xo, *uo;
+    if (j < tl) {
+      xo = state_traj + ((size_t)b * tl + j) * nd;
+      uo = input_traj + ((size_t)b * tl + j) * nd;
+    } else if (ideal) {
+      xo = M.pred_x + (size_t)b * nd;
+      uo = M.pred_u + (size_t)b * nd;
+    } else {
+      xo = nullptr;
+      uo = M.U + ((size_t)b * (M.n_samp + 1) + (j - tl)) * nd;
+    }
+    for (int c = 0; c < nd; ++c) {
+      if (xo) xo[c] = v[0][c];
+      uo[c] = v[1][c];
+    }
+  }
+  __syncthreads();                    // (every thread has read t_b)
+  if (t == 0) {
+    M.Tm[b] = T;
+    M.ns[b] = ns;
+    M.phase[b] = OMG_MPC_ACCEPTED;
+    M.t[b] = omg_round6(M.t[b] + M.update_time);
+  }
+}
+
+__global__ void omg_mpc_fill_kernel(int B, double v, double* __restrict__ out) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b < B) out[b] = v;
+}
+
 __global__ void omg_mpc_flag_kernel(int B, const int* __restrict__ mask, int* __restrict__ rec) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b < B && mask[b]) rec[b] = 1;
@@ -3476,6 +3728,7 @@ __global__ void omg_mpc_flag_kernel(int B, const int* __restrict__ mask, int* __
 
 struct omg_mpc {
   omg_problem* h = nullptr;
+  bool free_T = false;
   MpcDev M;
   size_t smem_prepare = 0, smem_commit = 0;
   std::vector<void*> allocs;
@@ -3499,82 +3752,32 @@ const MpcField kMpcFields[] = {
   MF(x_template, 3), MF(p_template, 3),
 };
 #undef MF
-struct OwnedMpc { omg_mpc_desc D; std::vector<void*> blocks; };
+#define MF(f, k) {#f, k, offsetof(omg_mpc_freeT_desc, f)}
+const MpcField kMpcFreeTFields[] = {
+  MF(n, 0), MF(n_par, 0), MF(n_dim, 0), MF(spl_offset, 0), MF(L, 0), MF(degree, 0), MF(knots, 3),
+  MF(update_time, 1), MF(sample_time, 1), MF(stop_tol, 1), MF(t_index, 0),
+  MF(p_state0, 0), MF(p_input0, 0), MF(p_poseT, 0),
+  MF(n_obs, 0), MF(obs_kind, 2), MF(obs_off, 2),
+  MF(n_blocks, 0), MF(blk_off, 2), MF(blk_len, 2), MF(blk_ncol, 2), MF(blk_degree, 2), MF(blk_knots, 3),
+  MF(x_template, 3), MF(p_template, 3),
+};
+#undef MF
+template <class D> struct OwnedDesc { D desc; std::vector<void*> blocks; };
 
-bool mpc_range(const std::string& what, int64_t lo, int64_t len, int64_t size) {
-  if (lo < 0 || len < 0 || lo + len > size) {
-    set_err("omg_mpc_create: " + what + " at " + std::to_string(lo) + " (+" + std::to_string(len) + ") outside [0, " +
-            std::to_string(size) + ")");
-    return false;
-  }
-  return true;
-}
-
-// Checks of omg_mpc_create; n_samp receives update_time / sample_time.
-bool mpc_check(const omg_problem* h, const omg_mpc_desc* D, int32_t B, int32_t traj_len, int32_t mode, int* n_samp) {
-  const std::string f("omg_mpc_create: ");
-  if (D->n != h->T.n || D->n_par != h->T.n_par) {
-    set_err(f + "the descriptor is for n = " + std::to_string(D->n) + ", n_par = " + std::to_string(D->n_par) +
-            ", the problem has n = " + std::to_string(h->T.n) + ", n_par = " + std::to_string(h->T.n_par));
-    return false;
-  }
-  if (B <= 0) { set_err(f + "B must be >= 1, got " + std::to_string(B)); return false; }
-  if (mode != OMG_MPC_PREDICT_IDEAL && mode != OMG_MPC_PREDICT_INTEGRATE) {
-    set_err(f + "unknown prediction " + std::to_string(mode)); return false; }
-  if (!(D->horizon > 0.0) || !(D->knot_time > 0.0) || !(D->sample_time > 0.0) || !(D->update_time > 0.0)) {
-    set_err(f + "horizon, knot_time, update_time and sample_time must be > 0"); return false; }
-  const double r = D->update_time / D->sample_time;
-  *n_samp = (int)rint(r);
-  if (*n_samp < 1 || fabs(r - *n_samp) > 1e-9 * std::max(1.0, r)) {
-    set_err(f + "update_time " + std::to_string(D->update_time) + " is not a multiple of sample_time " +
-            std::to_string(D->sample_time)); return false; }
-  const int max_len = (int)rint(D->horizon / D->sample_time * 1e6) / 1000000;
-  if (traj_len < 1 || traj_len > max_len) {
-    set_err(f + "trajectory_length " + std::to_string(traj_len) + " outside 1 .. horizon / sample_time = " +
-            std::to_string(max_len)); return false; }
-  const int nd = D->n_dim, L = D->L, p = D->degree;
-  if (nd < 1 || nd > OMG_CL_MAX_INPUT) { set_err(f + "n_dim must be 1 .. 3"); return false; }
-  if (p < 1 || p > OMG_SPL_MAX_DEGREE || L < p + 1 || L > OMG_SPL_MAX_LEN) {
-    set_err(f + "degree " + std::to_string(p) + " / basis length " + std::to_string(L) + " outside 1 <= p <= " +
-            std::to_string(OMG_SPL_MAX_DEGREE) + ", p + 1 <= L <= " + std::to_string(OMG_SPL_MAX_LEN)); return false; }
-  if (!D->knots || !D->x_template || !D->p_template || (D->n_obs > 0 && (!D->obs_kind || !D->obs_off)) ||
-      (D->n_shift > 0 && (!D->shift_off || !D->shift_len || !D->shift_ncol || !D->shift_T)) ||
-      D->n_obs < 0 || D->n_shift < 0) { set_err(f + "null descriptor array"); return false; }
-  for (int j = 0; j < L + p; ++j)
-    if (!(D->knots[j] <= D->knots[j + 1])) { set_err(f + "knots not non-decreasing"); return false; }
-  if (!mpc_range("vehicle splines", D->spl_offset, (int64_t)nd * L, D->n) ||
-      !mpc_range("state0", D->p_state0, nd, D->n_par) || !mpc_range("input0", D->p_input0, nd, D->n_par) ||
-      !mpc_range("poseT", D->p_poseT, nd, D->n_par) || !mpc_range("t", D->p_t, 1, D->n_par) ||
-      !mpc_range("T", D->p_T, 1, D->n_par)) return false;
-  for (int k = 0; k < D->n_obs; ++k) {
-    const std::string o = "obstacle " + std::to_string(k) + " ";
-    if (D->obs_kind[k] != 0 && D->obs_kind[k] != 1) { set_err(f + o + "kind must be 0 or 1"); return false; }
-    for (int q = 0; q < 3; ++q)
-      if (!mpc_range(o + "x/v/a", D->obs_off[4 * k + q], nd, D->n_par)) return false;
-    if (D->obs_kind[k] && !mpc_range(o + "theta", D->obs_off[4 * k + 3], 1, D->n_par)) return false;
-  }
-  for (int k = 0; k < D->n_shift; ++k)
-    if (D->shift_len[k] < 1 || D->shift_ncol[k] < 1 ||
-        !mpc_range("shift block " + std::to_string(k), D->shift_off[k], (int64_t)D->shift_len[k] * D->shift_ncol[k], D->n))
-      return false;
-  if (2 * (size_t)D->n * sizeof(double) > 227 * 1024) { set_err(f + "two x rows exceed the shared memory of a block"); return false; }
-  return true;
-}
-}  // namespace
-
-extern "C" {
-
-omg_mpc_desc* omg_mpc_read(const char* path) {
+// An MPC file of the fields `fields` into a heap descriptor; a record that is not one of them but one
+// of `other` (no) marks the other kind of MPC file, which `other_reader` reads.
+template <class D>
+D* mpc_read_file(const char* path, const MpcField* fields, int nf, const MpcField* other, int no,
+                 const char* other_reader) {
   FILE* fp = path ? fopen(path, "rb") : nullptr;
   if (!fp) { set_err(std::string("cannot open MPC file ") + (path ? path : "(null)")); return nullptr; }
-  OwnedMpc* O = new OwnedMpc();
-  memset(&O->D, 0, sizeof(O->D));
+  OwnedDesc<D>* O = new OwnedDesc<D>();
+  memset(&O->desc, 0, sizeof(O->desc));
   bool ok = true;
   char magic[8]; int32_t ver = 0, nrec = 0;
   if (fread(magic, 1, 8, fp) != 8 || memcmp(magic, "OMGMPC\0\0", 8) != 0) { set_err("not an omg MPC file"); ok = false; }
   if (ok && (fread(&ver, 4, 1, fp) != 1 || fread(&nrec, 4, 1, fp) != 1)) { set_err("truncated MPC file"); ok = false; }
   if (ok && ver != OMG_ABI_VERSION) { set_err("MPC file written for another ABI version"); ok = false; }
-  const int nf = (int)(sizeof(kMpcFields) / sizeof(kMpcFields[0]));
   std::vector<char> seen(nf, 0);
   for (int r = 0; ok && r < nrec; ++r) {
     char name[24]; int32_t dtype = 0, pad = 0; int64_t count = 0;
@@ -3582,11 +3785,15 @@ omg_mpc_desc* omg_mpc_read(const char* path) {
         fread(&count, 8, 1, fp) != 1 || count < 0) { set_err("truncated MPC file"); ok = false; break; }
     name[23] = 0;
     int k = -1;
-    for (int q = 0; q < nf; ++q) if (strcmp(kMpcFields[q].name, name) == 0) { k = q; break; }
-    const int kind = k < 0 ? -1 : kMpcFields[k].kind;
+    for (int q = 0; q < nf; ++q) if (strcmp(fields[q].name, name) == 0) { k = q; break; }
+    bool other_kind = false;
+    for (int q = 0; k < 0 && q < no; ++q) other_kind = other_kind || strcmp(other[q].name, name) == 0;
+    if (other_kind) {
+      set_err(std::string("this MPC file is of the other kind: read it with ") + other_reader); ok = false; break; }
+    const int kind = k < 0 ? -1 : fields[k].kind;
     if (k < 0 || dtype != (kind == 1 || kind == 3 ? 1 : 0)) { set_err(std::string("unknown record in MPC file: ") + name); ok = false; break; }
     const size_t esz = dtype ? 8 : 4;
-    char* base = reinterpret_cast<char*>(&O->D) + kMpcFields[k].off;
+    char* base = reinterpret_cast<char*>(&O->desc) + fields[k].off;
     if (kind < 2) {
       if (count != 1 || fread(base, esz, 1, fp) != 1) { set_err(std::string("bad scalar record ") + name); ok = false; break; }
     } else {
@@ -3599,17 +3806,132 @@ omg_mpc_desc* omg_mpc_read(const char* path) {
   }
   fclose(fp);
   for (int q = 0; ok && q < nf; ++q)
-    if (!seen[q]) { set_err(std::string("MPC file lacks ") + kMpcFields[q].name); ok = false; }
-  if (!ok) { omg_mpc_free_desc(&O->D); return nullptr; }
-  return &O->D;
+    if (!seen[q]) { set_err(std::string("MPC file lacks ") + fields[q].name); ok = false; }
+  if (!ok) { for (void* b : O->blocks) free(b); delete O; return nullptr; }
+  return &O->desc;
 }
 
-void omg_mpc_free_desc(omg_mpc_desc* desc) {
+template <class D> void mpc_free_file(D* desc) {
   if (!desc) return;
-  OwnedMpc* O = reinterpret_cast<OwnedMpc*>(desc);   // D is the first member
+  OwnedDesc<D>* O = reinterpret_cast<OwnedDesc<D>*>(desc);   // desc is the first member
   for (void* b : O->blocks) free(b);
   delete O;
 }
+
+bool mpc_range(const std::string& f, const std::string& what, int64_t lo, int64_t len, int64_t size) {
+  if (lo < 0 || len < 0 || lo + len > size) {
+    set_err(f + what + " at " + std::to_string(lo) + " (+" + std::to_string(len) + ") outside [0, " +
+            std::to_string(size) + ")");
+    return false;
+  }
+  return true;
+}
+
+// The checks both kinds of descriptor share (f: the message prefix); n_samp receives
+// update_time / sample_time.
+template <class D>
+bool mpc_check_common(const std::string& f, const omg_problem* h, const D* d, int32_t B, int32_t mode, int* n_samp) {
+  if (d->n != h->T.n || d->n_par != h->T.n_par) {
+    set_err(f + "the descriptor is for n = " + std::to_string(d->n) + ", n_par = " + std::to_string(d->n_par) +
+            ", the problem has n = " + std::to_string(h->T.n) + ", n_par = " + std::to_string(h->T.n_par));
+    return false;
+  }
+  if (B <= 0) { set_err(f + "B must be >= 1, got " + std::to_string(B)); return false; }
+  if (mode != OMG_MPC_PREDICT_IDEAL && mode != OMG_MPC_PREDICT_INTEGRATE) {
+    set_err(f + "unknown prediction " + std::to_string(mode)); return false; }
+  if (!(d->sample_time > 0.0) || !(d->update_time > 0.0)) {
+    set_err(f + "update_time and sample_time must be > 0"); return false; }
+  const double r = d->update_time / d->sample_time;
+  *n_samp = (int)rint(r);
+  if (*n_samp < 1 || fabs(r - *n_samp) > 1e-9 * std::max(1.0, r)) {
+    set_err(f + "update_time " + std::to_string(d->update_time) + " is not a multiple of sample_time " +
+            std::to_string(d->sample_time)); return false; }
+  const int nd = d->n_dim, L = d->L, p = d->degree;
+  if (nd < 1 || nd > OMG_CL_MAX_INPUT) { set_err(f + "n_dim must be 1 .. 3"); return false; }
+  if (p < 1 || p > OMG_SPL_MAX_DEGREE || L < p + 1 || L > OMG_SPL_MAX_LEN) {
+    set_err(f + "degree " + std::to_string(p) + " / basis length " + std::to_string(L) + " outside 1 <= p <= " +
+            std::to_string(OMG_SPL_MAX_DEGREE) + ", p + 1 <= L <= " + std::to_string(OMG_SPL_MAX_LEN)); return false; }
+  if (!d->knots || !d->x_template || !d->p_template || (d->n_obs > 0 && (!d->obs_kind || !d->obs_off)) ||
+      d->n_obs < 0) { set_err(f + "null descriptor array"); return false; }
+  for (int j = 0; j < L + p; ++j)
+    if (!(d->knots[j] <= d->knots[j + 1])) { set_err(f + "knots not non-decreasing"); return false; }
+  if (!mpc_range(f, "vehicle splines", d->spl_offset, (int64_t)nd * L, d->n) ||
+      !mpc_range(f, "state0", d->p_state0, nd, d->n_par) || !mpc_range(f, "input0", d->p_input0, nd, d->n_par) ||
+      !mpc_range(f, "poseT", d->p_poseT, nd, d->n_par)) return false;
+  for (int k = 0; k < d->n_obs; ++k) {
+    const std::string o = "obstacle " + std::to_string(k) + " ";
+    if (d->obs_kind[k] != 0 && d->obs_kind[k] != 1) { set_err(f + o + "kind must be 0 or 1"); return false; }
+    for (int q = 0; q < 3; ++q)
+      if (!mpc_range(f, o + "x/v/a", d->obs_off[4 * k + q], nd, d->n_par)) return false;
+    if (d->obs_kind[k] && !mpc_range(f, o + "theta", d->obs_off[4 * k + 3], 1, d->n_par)) return false;
+  }
+  return true;
+}
+
+// Checks of omg_mpc_create; n_samp receives update_time / sample_time.
+bool mpc_check(const omg_problem* h, const omg_mpc_desc* D, int32_t B, int32_t traj_len, int32_t mode, int* n_samp) {
+  const std::string f("omg_mpc_create: ");
+  if (!(D->horizon > 0.0) || !(D->knot_time > 0.0) || !(D->sample_time > 0.0) || !(D->update_time > 0.0)) {
+    set_err(f + "horizon, knot_time, update_time and sample_time must be > 0"); return false; }
+  if (!mpc_check_common(f, h, D, B, mode, n_samp)) return false;
+  const int max_len = (int)rint(D->horizon / D->sample_time * 1e6) / 1000000;
+  if (traj_len < 1 || traj_len > max_len) {
+    set_err(f + "trajectory_length " + std::to_string(traj_len) + " outside 1 .. horizon / sample_time = " +
+            std::to_string(max_len)); return false; }
+  if ((D->n_shift > 0 && (!D->shift_off || !D->shift_len || !D->shift_ncol || !D->shift_T)) || D->n_shift < 0) {
+    set_err(f + "null descriptor array"); return false; }
+  if (!mpc_range(f, "t", D->p_t, 1, D->n_par) || !mpc_range(f, "T", D->p_T, 1, D->n_par)) return false;
+  for (int k = 0; k < D->n_shift; ++k)
+    if (D->shift_len[k] < 1 || D->shift_ncol[k] < 1 ||
+        !mpc_range(f, "shift block " + std::to_string(k), D->shift_off[k], (int64_t)D->shift_len[k] * D->shift_ncol[k], D->n))
+      return false;
+  if (2 * (size_t)D->n * sizeof(double) > 227 * 1024) { set_err(f + "two x rows exceed the shared memory of a block"); return false; }
+  return true;
+}
+
+// Checks of omg_mpc_create_freet; n_samp as above, iv / n_knots / Lmax / pmax: the block
+// descriptor of spline_desc.
+bool mpc_check_freeT(const omg_problem* h, const omg_mpc_freeT_desc* D, int32_t B, int32_t traj_len, int32_t mode,
+                     int* n_samp, std::vector<int>& iv, size_t* n_knots, int* Lmax, int* pmax) {
+  const std::string f("omg_mpc_create_freet: ");
+  if (!mpc_check_common(f, h, D, B, mode, n_samp)) return false;
+  if (!(D->stop_tol >= 0.0)) { set_err(f + "stop_tol must be >= 0"); return false; }
+  if (D->t_index < 0 || D->t_index >= D->n) {
+    set_err(f + "t_index " + std::to_string(D->t_index) + " outside [0, " + std::to_string(D->n) + ")"); return false; }
+  const double T = D->x_template[D->t_index];
+  const int max_len = T > 0.0 ? (int)rint(T / D->sample_time * 1e6) / 1000000 : 0;
+  if (traj_len < 1 || traj_len > max_len) {
+    set_err(f + "trajectory_length " + std::to_string(traj_len) + " outside 1 .. (template T) / sample_time = " +
+            std::to_string(max_len)); return false; }
+  if (D->n_blocks < 0 || (D->n_blocks > 0 && (!D->blk_off || !D->blk_len || !D->blk_ncol || !D->blk_degree ||
+                                              !D->blk_knots))) { set_err(f + "null descriptor array"); return false; }
+  size_t n_coef = 0;
+  if (!spline_desc("omg_mpc_create_freet", D->n, D->n_blocks, D->blk_off, D->blk_len, D->blk_ncol, D->blk_degree,
+                   D->blk_knots, 1, iv, n_knots, Lmax, pmax, &n_coef)) return false;
+  const size_t smem = sizeof(double) * (2 * (size_t)D->n + 2 * (size_t)*Lmax + *pmax + 1 + 2 * OMG_MPC_NT +
+                                        2 * (size_t)*Lmax * *Lmax);
+  if (smem > 227 * 1024) { set_err(f + "two x rows and the shift's bases exceed the shared memory of a block"); return false; }
+  return true;
+}
+}  // namespace
+
+extern "C" {
+
+omg_mpc_desc* omg_mpc_read(const char* path) {
+  const int nf = (int)(sizeof(kMpcFields) / sizeof(kMpcFields[0]));
+  const int no = (int)(sizeof(kMpcFreeTFields) / sizeof(kMpcFreeTFields[0]));
+  return mpc_read_file<omg_mpc_desc>(path, kMpcFields, nf, kMpcFreeTFields, no, "omg_mpc_freet_read");
+}
+
+void omg_mpc_free_desc(omg_mpc_desc* desc) { mpc_free_file(desc); }
+
+omg_mpc_freeT_desc* omg_mpc_freet_read(const char* path) {
+  const int nf = (int)(sizeof(kMpcFreeTFields) / sizeof(kMpcFreeTFields[0]));
+  const int no = (int)(sizeof(kMpcFields) / sizeof(kMpcFields[0]));
+  return mpc_read_file<omg_mpc_freeT_desc>(path, kMpcFreeTFields, nf, kMpcFields, no, "omg_mpc_read");
+}
+
+void omg_mpc_freet_release(omg_mpc_freeT_desc* desc) { mpc_free_file(desc); }
 
 void omg_mpc_destroy(omg_mpc* mpc) {
   if (!mpc) return;
@@ -3618,69 +3940,117 @@ void omg_mpc_destroy(omg_mpc* mpc) {
   delete mpc;
 }
 
+}  // extern "C"
+
+namespace {
+// A device buffer of the handle, a copy of src (or zeros); *ok turns false on failure.
+void* mpc_alloc(omg_mpc* q, size_t bytes, const void* src, bool* ok) {
+  void* d = nullptr;
+  if (cudaMalloc(&d, bytes ? bytes : 8) != cudaSuccess) { *ok = false; return nullptr; }
+  q->allocs.push_back(d);
+  if (src && bytes && cudaMemcpy(d, src, bytes, cudaMemcpyHostToDevice) != cudaSuccess) *ok = false;
+  else if (!src && cudaMemset(d, 0, bytes ? bytes : 8) != cudaSuccess) *ok = false;
+  return d;
+}
+
+// The handle's fields and buffers both kinds of descriptor share.
+template <class D>
+omg_mpc* mpc_new(omg_problem* h, const D* d, int32_t B, int32_t traj_len, int32_t mode, int n_samp, bool* ok) {
+  omg_mpc* q = new omg_mpc();
+  q->h = h;
+  MpcDev& M = q->M;
+  memset(&M, 0, sizeof(M));
+  const int n = d->n, np_ = d->n_par, nd = d->n_dim, L = d->L, p = d->degree;
+  M.B = B; M.n = n; M.n_par = np_; M.nd = nd; M.spl_off = d->spl_offset; M.L = L; M.p = p;
+  M.traj_len = traj_len; M.n_samp = n_samp; M.mode = mode; M.n_obs = d->n_obs;
+  M.p_state0 = d->p_state0; M.p_input0 = d->p_input0; M.p_poseT = d->p_poseT;
+  M.update_time = d->update_time; M.sample_time = d->sample_time;
+  const size_t b = B, d8 = sizeof(double);
+  M.knots = (const double*)mpc_alloc(q, d8 * (L + p + 1), d->knots, ok);
+  M.obs_kind = (const int*)mpc_alloc(q, 4 * (size_t)d->n_obs, d->obs_kind, ok);
+  M.obs_off = (const int*)mpc_alloc(q, 16 * (size_t)d->n_obs, d->obs_off, ok);
+  M.x_tpl = (const double*)mpc_alloc(q, d8 * n, d->x_template, ok);
+  M.p_tpl = (const double*)mpc_alloc(q, d8 * np_, d->p_template, ok);
+  M.X = (double*)mpc_alloc(q, d8 * b * n, nullptr, ok);
+  M.X0 = (double*)mpc_alloc(q, d8 * b * n, nullptr, ok);
+  M.Xn = (double*)mpc_alloc(q, d8 * b * n, nullptr, ok);
+  M.P = (double*)mpc_alloc(q, d8 * b * np_, nullptr, ok);
+  M.t = (double*)mpc_alloc(q, d8 * b, nullptr, ok);
+  M.pred_x = (double*)mpc_alloc(q, d8 * b * nd, nullptr, ok);
+  M.pred_u = (double*)mpc_alloc(q, d8 * b * nd, nullptr, ok);
+  M.U = (double*)mpc_alloc(q, d8 * b * (n_samp + 1) * nd, nullptr, ok);
+  M.rec = (int*)mpc_alloc(q, 4 * b, nullptr, ok);
+  q->lam = (double*)mpc_alloc(q, d8 * b * h->T.m, nullptr, ok);
+  q->f = (double*)mpc_alloc(q, d8 * b, nullptr, ok);
+  q->mask = (int*)mpc_alloc(q, 4 * b, nullptr, ok);
+  q->s0 = (double*)mpc_alloc(q, d8 * b * nd, nullptr, ok);
+  q->sT = (double*)mpc_alloc(q, d8 * b * nd, nullptr, ok);
+  q->obs = (double*)mpc_alloc(q, d8 * b * d->n_obs * (3 * nd + 1), nullptr, ok);
+  q->xtraj = (double*)mpc_alloc(q, d8 * b * traj_len * nd, nullptr, ok);
+  q->utraj = (double*)mpc_alloc(q, d8 * b * traj_len * nd, nullptr, ok);
+  q->st = (int*)mpc_alloc(q, 4 * b, nullptr, ok);
+  q->it = (int*)mpc_alloc(q, 4 * b, nullptr, ok);
+  q->smem_commit = 2 * d8 * nd * L;
+  return q;
+}
+}  // namespace
+
+extern "C" {
+
 omg_mpc* omg_mpc_create(omg_problem* h, const omg_mpc_desc* D, int32_t B, int32_t traj_len, int32_t mode) {
   if (!h || !D) { set_err("omg_mpc_create: null argument"); return nullptr; }
   int n_samp = 0;
   if (!mpc_check(h, D, B, traj_len, mode, &n_samp)) return nullptr;
   if (cudaSetDevice(h->device) != cudaSuccess) { set_err("omg_mpc_create: cudaSetDevice failed"); return nullptr; }
-  omg_mpc* q = new omg_mpc();
-  q->h = h;
-  MpcDev& M = q->M;
-  memset(&M, 0, sizeof(M));
-  const int n = D->n, np_ = D->n_par, nd = D->n_dim, L = D->L, p = D->degree;
-  M.B = B; M.n = n; M.n_par = np_; M.nd = nd; M.spl_off = D->spl_offset; M.L = L; M.p = p;
-  M.traj_len = traj_len; M.n_samp = n_samp; M.mode = mode; M.n_obs = D->n_obs; M.n_shift = D->n_shift;
-  M.p_state0 = D->p_state0; M.p_input0 = D->p_input0; M.p_poseT = D->p_poseT; M.p_t = D->p_t; M.p_T = D->p_T;
-  M.horizon = D->horizon; M.knot_time = D->knot_time; M.update_time = D->update_time; M.sample_time = D->sample_time;
   bool ok = true;
-  auto alloc = [&](size_t bytes, const void* src) -> void* {
-    void* d = nullptr;
-    if (cudaMalloc(&d, bytes ? bytes : 8) != cudaSuccess) { ok = false; return nullptr; }
-    q->allocs.push_back(d);
-    if (src && bytes && cudaMemcpy(d, src, bytes, cudaMemcpyHostToDevice) != cudaSuccess) ok = false;
-    else if (!src && cudaMemset(d, 0, bytes ? bytes : 8) != cudaSuccess) ok = false;
-    return d;
-  };
+  omg_mpc* q = mpc_new(h, D, B, traj_len, mode, n_samp, &ok);
+  MpcDev& M = q->M;
+  M.n_shift = D->n_shift; M.p_t = D->p_t; M.p_T = D->p_T;
+  M.horizon = D->horizon; M.knot_time = D->knot_time;
   std::vector<int> sd(4 * (size_t)D->n_shift);
   size_t nT = 0;
   for (int k = 0; k < D->n_shift; ++k) {
     sd[4 * k] = D->shift_off[k]; sd[4 * k + 1] = D->shift_len[k]; sd[4 * k + 2] = D->shift_ncol[k]; sd[4 * k + 3] = (int)nT;
     nT += (size_t)D->shift_len[k] * D->shift_len[k];
   }
-  const size_t b = B, d8 = sizeof(double);
-  M.knots = (const double*)alloc(d8 * (L + p + 1), D->knots);
-  M.obs_kind = (const int*)alloc(4 * (size_t)D->n_obs, D->obs_kind);
-  M.obs_off = (const int*)alloc(16 * (size_t)D->n_obs, D->obs_off);
-  M.shift_desc = (const int*)alloc(4 * sd.size(), sd.data());
-  M.shift_T = (const double*)alloc(d8 * nT, D->shift_T);
-  M.x_tpl = (const double*)alloc(d8 * n, D->x_template);
-  M.p_tpl = (const double*)alloc(d8 * np_, D->p_template);
-  M.X = (double*)alloc(d8 * b * n, nullptr);
-  M.X0 = (double*)alloc(d8 * b * n, nullptr);
-  M.Xn = (double*)alloc(d8 * b * n, nullptr);
-  M.P = (double*)alloc(d8 * b * np_, nullptr);
-  M.t = (double*)alloc(d8 * b, nullptr);
-  M.t_prev = (double*)alloc(d8 * b, nullptr);
-  M.pred_x = (double*)alloc(d8 * b * nd, nullptr);
-  M.pred_u = (double*)alloc(d8 * b * nd, nullptr);
-  M.U = (double*)alloc(d8 * b * (n_samp + 1) * nd, nullptr);
-  M.rec = (int*)alloc(4 * b, nullptr);
-  q->lam = (double*)alloc(d8 * b * h->T.m, nullptr);
-  q->f = (double*)alloc(d8 * b, nullptr);
-  q->mask = (int*)alloc(4 * b, nullptr);
-  q->s0 = (double*)alloc(d8 * b * nd, nullptr);
-  q->sT = (double*)alloc(d8 * b * nd, nullptr);
-  q->obs = (double*)alloc(d8 * b * D->n_obs * (3 * nd + 1), nullptr);
-  q->xtraj = (double*)alloc(d8 * b * traj_len * nd, nullptr);
-  q->utraj = (double*)alloc(d8 * b * traj_len * nd, nullptr);
-  q->st = (int*)alloc(4 * b, nullptr);
-  q->it = (int*)alloc(4 * b, nullptr);
-  q->smem_prepare = 2 * d8 * n;
-  q->smem_commit = 2 * d8 * nd * L;
+  M.shift_desc = (const int*)mpc_alloc(q, 4 * sd.size(), sd.data(), &ok);
+  M.shift_T = (const double*)mpc_alloc(q, sizeof(double) * nT, D->shift_T, &ok);
+  M.t_prev = (double*)mpc_alloc(q, sizeof(double) * B, nullptr, &ok);
+  q->smem_prepare = 2 * sizeof(double) * D->n;
   if (ok && q->smem_prepare > 48 * 1024 &&
       cudaFuncSetAttribute((const void*)omg_mpc_prepare_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                            (int)q->smem_prepare) != cudaSuccess) ok = false;
   if (!ok) { set_err("omg_mpc_create: device allocation/upload failed"); omg_mpc_destroy(q); return nullptr; }
+  return q;
+}
+
+omg_mpc* omg_mpc_create_freet(omg_problem* h, const omg_mpc_freeT_desc* D, int32_t B, int32_t traj_len, int32_t mode) {
+  if (!h || !D) { set_err("omg_mpc_create_freet: null argument"); return nullptr; }
+  int n_samp = 0, Lmax = 1, pmax = 0;
+  std::vector<int> iv;
+  size_t n_knots = 0;
+  if (!mpc_check_freeT(h, D, B, traj_len, mode, &n_samp, iv, &n_knots, &Lmax, &pmax)) return nullptr;
+  if (cudaSetDevice(h->device) != cudaSuccess) { set_err("omg_mpc_create_freet: cudaSetDevice failed"); return nullptr; }
+  bool ok = true;
+  omg_mpc* q = mpc_new(h, D, B, traj_len, mode, n_samp, &ok);
+  q->free_T = true;
+  MpcDev& M = q->M;
+  M.t_index = D->t_index; M.n_blocks = D->n_blocks; M.Lmax = Lmax; M.pmax = pmax; M.stop_tol = D->stop_tol;
+  M.blk_desc = (const int*)mpc_alloc(q, 4 * iv.size(), iv.data(), &ok);
+  M.blk_knots = (const double*)mpc_alloc(q, sizeof(double) * n_knots, D->blk_knots, &ok);
+  const std::vector<double> T0(B, D->x_template[D->t_index]);
+  M.Tm = (double*)mpc_alloc(q, sizeof(double) * B, T0.data(), &ok);
+  M.phase = (int*)mpc_alloc(q, 4 * (size_t)B, nullptr, &ok);
+  M.stop = (int*)mpc_alloc(q, 4 * (size_t)B, nullptr, &ok);
+  M.ns = (int*)mpc_alloc(q, 4 * (size_t)B, nullptr, &ok);
+  M.rows = (int*)mpc_alloc(q, 4 * (size_t)B, nullptr, &ok);
+  M.n_rows = (int*)mpc_alloc(q, 4, nullptr, &ok);
+  q->smem_prepare = sizeof(double) * (2 * (size_t)D->n + 2 * (size_t)Lmax + pmax + 1 + 2 * OMG_MPC_NT +
+                                      2 * (size_t)Lmax * Lmax);
+  if (ok && q->smem_prepare > 48 * 1024 &&
+      cudaFuncSetAttribute((const void*)omg_mpc_prepare_free_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                           (int)q->smem_prepare) != cudaSuccess) ok = false;
+  if (!ok) { set_err("omg_mpc_create_freet: device allocation/upload failed"); omg_mpc_destroy(q); return nullptr; }
   return q;
 }
 
@@ -3692,6 +4062,19 @@ int omg_mpc_update(omg_mpc* q, const double* state0, const double* stateT, const
   omg_problem* h = q->h;
   CK(cudaSetDevice(h->device));
   const int B = q->M.B;
+  if (q->free_T) {
+    OMG_LAUNCH(omg_mpc_prepare_free_kernel, B, OMG_MPC_NT, q->smem_prepare, stream, q->M, state0, stateT, obstacles);
+    CK(cudaGetLastError());
+    OMG_LAUNCH(omg_mpc_rows_kernel, 1, 256, 256 * sizeof(int), stream, B, q->M.stop, q->M.rows, q->M.n_rows);
+    CK(cudaGetLastError());
+    if (solve_batch_rows(h, B, q->M.X0, q->M.P, h->lbg, h->ubg, 1, nullptr, q->M.Xn, q->lam, q->f, status, iters,
+                         q->M.rows, q->M.n_rows, stream))
+      return -1;
+    OMG_LAUNCH(omg_mpc_commit_free_kernel, B, OMG_MPC_NT, q->smem_commit, stream, q->M, status, iters, state_traj,
+               input_traj);
+    CK(cudaGetLastError());
+    return 0;
+  }
   OMG_LAUNCH(omg_mpc_prepare_kernel, B, OMG_MPC_NT, q->smem_prepare, stream, q->M, state0, stateT, obstacles);
   CK(cudaGetLastError());
   if (omg_solve_batch(h, B, q->M.X0, q->M.P, h->lbg, h->ubg, 1, nullptr, q->M.Xn, q->lam, q->f, status, iters, stream))
@@ -3736,6 +4119,19 @@ int omg_mpc_time(omg_mpc* q, double* t_out) {
   CK(cudaSetDevice(q->h->device));
   CK(cudaDeviceSynchronize());
   CK(cudaMemcpy(t_out, q->M.t, (size_t)q->M.B * 8, cudaMemcpyDeviceToHost));
+  return 0;
+}
+
+int omg_mpc_motion_time(omg_mpc* q, double* T_out, void* stream_) {
+  if (!q || !T_out) { set_err("omg_mpc_motion_time: null argument"); return -1; }
+  cudaStream_t stream = (cudaStream_t)stream_;
+  CK(cudaSetDevice(q->h->device));
+  const int B = q->M.B;
+  if (q->free_T) CK(cudaMemcpyAsync(T_out, q->M.Tm, (size_t)B * 8, cudaMemcpyDeviceToDevice, stream));
+  else {
+    OMG_LAUNCH(omg_mpc_fill_kernel, (B + 127) / 128, 128, 0, stream, B, q->M.horizon, T_out);
+    CK(cudaGetLastError());
+  }
   return 0;
 }
 

@@ -1008,7 +1008,7 @@ __device__ __forceinline__ void ipm_body_sp(const DevTab& T, const SpTab& P, con
   __syncthreads();
 
   for (;;) {
-    if (tid == 0) ctl.inst = atomicAdd(A.counter, 1);
+    if (tid == 0) ctl.inst = omg_next_row(A);
     __syncthreads();
     const int inst = ctl.inst;
     if (inst >= A.B) return;

@@ -10,6 +10,13 @@ state (read on a cold start, and by the 'integrate' prediction), the goal and th
 current x, v, a (and theta), as the reference's obstacle_t, and receives the planned state and
 input trajectories.  An update makes no synchronous CUDA call and no allocation after the first
 one, so a sequence of updates can be captured in a CUDA graph.
+
+With a FreeTPoint2point (the motion time T a decision variable) every instance runs the reference's
+free-T loop on its own T (include/omg_b200.h, omg_mpc_create_freet): the warm start is re-expressed
+from the plan's own T, the prediction and the trajectory samples are taken on the plan's own time
+axis, and an instance whose plan is shorter than update_time, or that has arrived at its goal, stops:
+it is not solved again (status MPC_STOPPED = -1, 0 iterations) until recover().  motion_time() gives
+each instance's T, and so how much of the returned trajectory is plan.
 """
 import ctypes as C
 
@@ -35,20 +42,27 @@ class DeviceMPC(object):
         import torch
         if prediction not in b200.MPC_PREDICTION:
             raise ValueError('prediction must be one of %s' % sorted(b200.MPC_PREDICTION))
-        desc = b200.mpc_desc(problem, update_time, sample_time)
+        from ..problems.point2point import FreeTPoint2point
+        self.free_T = isinstance(problem, FreeTPoint2point)
+        if self.free_T:
+            desc = b200.mpc_freeT_desc(problem, update_time, sample_time)
+            horizon, pack, create = desc['x_template'][desc['t_index']], b200.pack_mpc_freeT_desc, 'omg_mpc_create_freet'
+        else:
+            desc = b200.mpc_desc(problem, update_time, sample_time)
+            horizon, pack, create = desc['horizon'], b200.pack_mpc_desc, 'omg_mpc_create'
         self.solver = problem.problem
         self.lib = self.solver.lib
         self.B, self.n_dim, self.n_obs = int(batch), desc['n_dim'], desc['n_obs']
         if trajectory_length is None:
-            trajectory_length = int(np.round(desc['horizon'] / sample_time, 6))
+            trajectory_length = int(np.round(horizon / sample_time, 6))
         self.trajectory_length = int(trajectory_length)
         self.dev = device if device is not None else torch.device('cuda', self.solver.device)
-        D, keep = b200.pack_mpc_desc(desc)
-        self._handle = self.lib.omg_mpc_create(self.solver._handle, C.byref(D), self.B, self.trajectory_length,
-                                               b200.MPC_PREDICTION[prediction])
+        D, keep = pack(desc)
+        self._handle = getattr(self.lib, create)(self.solver._handle, C.byref(D), self.B, self.trajectory_length,
+                                                 b200.MPC_PREDICTION[prediction])
         del keep
         if not self._handle:
-            raise RuntimeError('omg_mpc_create failed: %s' % self.lib.omg_last_error().decode())
+            raise RuntimeError('%s failed: %s' % (create, self.lib.omg_last_error().decode()))
         self.n, self.n_par = desc['n'], desc['n_par']
         f64 = dict(dtype=torch.float64, device=self.dev)
         i32 = dict(dtype=torch.int32, device=self.dev)
@@ -90,6 +104,16 @@ class DeviceMPC(object):
         t = np.empty(self.B)
         self._check(self.lib.omg_mpc_time(self._handle, t.ctypes.data))
         return t
+
+    def motion_time(self, stream=None):
+        """Every instance's motion time T of its last accepted plan (the template's before the first;
+        the horizon with a fixed horizon): device tensor [B], without synchronising."""
+        import torch
+        T = torch.empty(self.B, dtype=torch.float64, device=self.dev)
+        on_gpu = b200._check_device_tensors((T,), self.lib)
+        self._check(self.lib.omg_mpc_motion_time(self._handle, T.data_ptr(),
+                                                 b200._stream_handle(on_gpu, T.device, stream)))
+        return T
 
     def last_problem(self, stream=None):
         """The warm start and parameter rows handed to the last solve: device tensors [B, n], [B, n_par]."""

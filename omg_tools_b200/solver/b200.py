@@ -93,7 +93,20 @@ class _MpcDesc(C.Structure):
     _fields_ = [(name, _CTYPE[kind]) for name, kind in MPC_FIELDS]
 
 
+# include/omg_b200.h omg_mpc_freeT_desc, in the same notation
+MPC_FREET_FIELDS = [('n', 'i'), ('n_par', 'i'), ('n_dim', 'i'), ('spl_offset', 'i'), ('L', 'i'), ('degree', 'i'),
+                    ('knots', 'D'), ('update_time', 'd'), ('sample_time', 'd'), ('stop_tol', 'd'), ('t_index', 'i'),
+                    ('p_state0', 'i'), ('p_input0', 'i'), ('p_poseT', 'i'), ('n_obs', 'i'), ('obs_kind', 'I'),
+                    ('obs_off', 'I'), ('n_blocks', 'i'), ('blk_off', 'I'), ('blk_len', 'I'), ('blk_ncol', 'I'),
+                    ('blk_degree', 'I'), ('blk_knots', 'D'), ('x_template', 'D'), ('p_template', 'D')]
+
+
+class _MpcFreeTDesc(C.Structure):
+    _fields_ = [(name, _CTYPE[kind]) for name, kind in MPC_FREET_FIELDS]
+
+
 MPC_PREDICTION = {'ideal': 0, 'integrate': 1}
+MPC_STOPPED = -1        # status of an instance that was not solved because it has stopped
 
 EXPORTS = ['omg_abi_version', 'omg_last_error', 'omg_default_options',
            'omg_problem_create', 'omg_problem_destroy', 'omg_set_options',
@@ -105,7 +118,9 @@ EXPORTS = ['omg_abi_version', 'omg_last_error', 'omg_default_options',
            'omg_admm_zl_update_dist', 'omg_closed_loop_step', 'omg_closed_loop_step_der',
            'omg_shift_free_batch', 'omg_eval_batch', 'omg_closed_loop_step_free', 'omg_closed_loop_step_fleet',
            'omg_mpc_read', 'omg_mpc_free_desc', 'omg_mpc_create', 'omg_mpc_destroy', 'omg_mpc_update',
-           'omg_mpc_update_host', 'omg_mpc_recover', 'omg_mpc_time', 'omg_mpc_last_problem']
+           'omg_mpc_update_host', 'omg_mpc_recover', 'omg_mpc_time', 'omg_mpc_last_problem',
+           'omg_mpc_freet_read', 'omg_mpc_freet_release', 'omg_mpc_create_freet', 'omg_mpc_motion_time',
+           'omg_solve_batch_rows']
 
 _lib = None
 
@@ -189,6 +204,14 @@ def bind(lib):
     lib.omg_mpc_recover.argtypes = [vp, vp]
     lib.omg_mpc_time.argtypes = [vp, vp]
     lib.omg_mpc_last_problem.argtypes = [vp] * 4
+    lib.omg_mpc_freet_read.argtypes = [C.c_char_p]
+    lib.omg_mpc_freet_read.restype = C.POINTER(_MpcFreeTDesc)
+    lib.omg_mpc_freet_release.argtypes = [C.POINTER(_MpcFreeTDesc)]
+    lib.omg_mpc_freet_release.restype = None
+    lib.omg_mpc_create_freet.argtypes = [vp, C.POINTER(_MpcFreeTDesc), C.c_int32, C.c_int32, C.c_int32]
+    lib.omg_mpc_create_freet.restype = C.c_void_p
+    lib.omg_mpc_motion_time.argtypes = [vp] * 3
+    lib.omg_solve_batch_rows.argtypes = [vp, C.c_int32, vp, vp, vp, vp, C.c_int32, vp] + [vp] * 8
     lib.omg_tables_read.argtypes = [C.c_char_p]
     lib.omg_tables_read.restype = C.POINTER(_Tables)
     lib.omg_tables_free.argtypes = [C.POINTER(_Tables)]
@@ -377,14 +400,9 @@ def save_tables(tb, path):
             fp.write(a.tobytes())
 
 
-def mpc_desc(problem, update_time=0.1, sample_time=0.01):
-    """The descriptor of the device-resident MPC update (include/omg_b200.h, omg_mpc_desc) of a
-    fixed-horizon Point2point with one Holonomic or Holonomic3D vehicle, as a dict of the
-    MPC_FIELDS.  Raises NotImplementedError naming the cause for anything else."""
-    from ..problems.point2point import FreeTPoint2point
-    if isinstance(problem, FreeTPoint2point):
-        raise NotImplementedError('the device MPC update has a fixed horizon only, not a free motion time '
-                                  '(FreeTPoint2point)')
+def _mpc_vehicle(problem):
+    """The vehicle, parameter and variable entries and obstacle records both device MPC descriptors
+    share; raises NotImplementedError naming the cause for what the device MPC update does not run."""
     if len(problem.vehicles) != 1:
         raise NotImplementedError('the device MPC update runs one vehicle, this problem has %d'
                                   % len(problem.vehicles))
@@ -407,50 +425,105 @@ def mpc_desc(problem, update_time=0.1, sample_time=0.01):
         rot = (o.label, 'theta') in par
         kind.append(int(rot))
         off.append([par[(o.label, k)][0] for k in ('x', 'v', 'a')] + [par[(o.label, 'theta')][0] if rot else -1])
-    shifted = father.shifted_entries()
-    lab, basis = problem.label, veh.basis
-    return {
+    basis = veh.basis
+    return veh, par, var, {
         'n': father.tables.n, 'n_par': father.tables.n_par, 'n_dim': nd,
         'spl_offset': var[(veh.label, 'splines_seg0')][0], 'L': len(basis), 'degree': basis.degree,
         'knots': np.asarray(basis.knots, dtype=np.float64),
-        'horizon': float(problem.options['horizon_time']), 'knot_time': float(problem.knot_time),
-        'update_time': float(update_time), 'sample_time': float(sample_time),
         'p_state0': par[(veh.label, 'state0')][0], 'p_input0': par[(veh.label, 'input0')][0],
-        'p_poseT': par[(veh.label, 'poseT')][0], 'p_t': par[(lab, 't')][0], 'p_T': par[(lab, 'T')][0],
+        'p_poseT': par[(veh.label, 'poseT')][0],
         'n_obs': len(kind), 'obs_kind': np.array(kind, dtype=np.int32),
         'obs_off': np.array(off, dtype=np.int32).reshape(-1),
-        'n_shift': len(shifted), 'shift_off': np.array([e[2] for e in shifted], dtype=np.int32),
-        'shift_len': np.array([e[3][0] for e in shifted], dtype=np.int32),
-        'shift_ncol': np.array([e[3][1] for e in shifted], dtype=np.int32),
-        'shift_T': np.concatenate([np.asarray(e[4], dtype=np.float64).reshape(-1) for e in shifted] + [np.zeros(0)]),
         'x_template': np.asarray(father.get_variables().cat, dtype=np.float64),
         'p_template': np.asarray(father.set_parameters(0.).cat, dtype=np.float64)}
 
 
-def pack_mpc_desc(desc):
-    """mpc_desc dict -> (ctypes omg_mpc_desc, keep-alive object)."""
-    keep, D = _Keep(), _MpcDesc()
-    for name, kind in MPC_FIELDS:
+def mpc_desc(problem, update_time=0.1, sample_time=0.01):
+    """The descriptor of the device-resident MPC update (include/omg_b200.h, omg_mpc_desc) of a
+    fixed-horizon Point2point with one Holonomic or Holonomic3D vehicle, as a dict of the
+    MPC_FIELDS.  Raises NotImplementedError naming the cause for anything else (mpc_freeT_desc
+    describes a free motion time)."""
+    from ..problems.point2point import FreeTPoint2point
+    if isinstance(problem, FreeTPoint2point):
+        raise NotImplementedError('the device MPC update has a fixed horizon only, not a free motion time '
+                                  '(FreeTPoint2point)')
+    veh, par, var, desc = _mpc_vehicle(problem)
+    shifted = problem.father.shifted_entries()
+    lab = problem.label
+    desc.update({
+        'horizon': float(problem.options['horizon_time']), 'knot_time': float(problem.knot_time),
+        'update_time': float(update_time), 'sample_time': float(sample_time),
+        'p_t': par[(lab, 't')][0], 'p_T': par[(lab, 'T')][0],
+        'n_shift': len(shifted), 'shift_off': np.array([e[2] for e in shifted], dtype=np.int32),
+        'shift_len': np.array([e[3][0] for e in shifted], dtype=np.int32),
+        'shift_ncol': np.array([e[3][1] for e in shifted], dtype=np.int32),
+        'shift_T': np.concatenate([np.asarray(e[4], dtype=np.float64).reshape(-1) for e in shifted] + [np.zeros(0)])})
+    return desc
+
+
+def mpc_freeT_desc(problem, update_time=0.1, sample_time=0.01):
+    """The descriptor of the device-resident MPC update with a free motion time (include/omg_b200.h,
+    omg_mpc_freeT_desc) of a FreeTPoint2point with one Holonomic or Holonomic3D vehicle, as a dict
+    of the MPC_FREET_FIELDS.  Raises NotImplementedError naming the cause for anything else."""
+    from ..problems.point2point import FreeTPoint2point
+    if not isinstance(problem, FreeTPoint2point):
+        raise NotImplementedError('mpc_freeT_desc describes a free motion time (FreeTPoint2point); '
+                                  'mpc_desc describes a fixed horizon')
+    veh, par, var, desc = _mpc_vehicle(problem)
+    blocks = spline_blocks(problem.father)
+    desc.update({
+        'update_time': float(update_time), 'sample_time': float(sample_time),
+        'stop_tol': float(veh.options['stop_tol']), 't_index': var[(problem.label, 'T')][0],
+        'n_blocks': len(blocks), 'blk_off': np.array([b[0] for b in blocks], dtype=np.int32),
+        'blk_len': np.array([b[1] for b in blocks], dtype=np.int32),
+        'blk_ncol': np.array([b[2] for b in blocks], dtype=np.int32),
+        'blk_degree': np.array([b[3] for b in blocks], dtype=np.int32),
+        'blk_knots': np.concatenate([np.asarray(b[4], dtype=np.float64) for b in blocks] + [np.zeros(0)])})
+    return desc
+
+
+def _pack(desc, fields, cls):
+    keep, D = _Keep(), cls()
+    for name, kind in fields:
         v = desc[name]
         cast = {'i': int, 'd': float, 'I': keep.i32, 'D': keep.f64}[kind]
         setattr(D, name, cast(v))
     return D, keep
 
 
-def save_mpc(problem, path, update_time=0.1, sample_time=0.01):
-    """Write the descriptor of the device MPC update to an MPC file (include/omg_b200.h:
-    omg_mpc_read), the companion of save_tables for native callers of omg_mpc_update."""
+def pack_mpc_desc(desc):
+    """mpc_desc dict -> (ctypes omg_mpc_desc, keep-alive object)."""
+    return _pack(desc, MPC_FIELDS, _MpcDesc)
+
+
+def pack_mpc_freeT_desc(desc):
+    """mpc_freeT_desc dict -> (ctypes omg_mpc_freeT_desc, keep-alive object)."""
+    return _pack(desc, MPC_FREET_FIELDS, _MpcFreeTDesc)
+
+
+def _write_mpc(desc, fields, path):
     import struct
-    desc = mpc_desc(problem, update_time, sample_time)
     with open(path, 'wb') as fp:
         fp.write(b'OMGMPC\0\0')
-        fp.write(struct.pack('<ii', ABI_VERSION, len(MPC_FIELDS)))
-        for name, kind in MPC_FIELDS:
+        fp.write(struct.pack('<ii', ABI_VERSION, len(fields)))
+        for name, kind in fields:
             dtype = 1 if kind in 'dD' else 0
             a = np.ascontiguousarray(desc[name], dtype=np.float64 if dtype else np.int32).reshape(-1)
             fp.write(name.encode().ljust(24, b'\0'))
             fp.write(struct.pack('<iiq', dtype, 0, a.size))
             fp.write(a.tobytes())
+
+
+def save_mpc(problem, path, update_time=0.1, sample_time=0.01):
+    """Write the descriptor of the device MPC update to an MPC file (include/omg_b200.h:
+    omg_mpc_read), the companion of save_tables for native callers of omg_mpc_update."""
+    _write_mpc(mpc_desc(problem, update_time, sample_time), MPC_FIELDS, path)
+
+
+def save_mpc_freeT(problem, path, update_time=0.1, sample_time=0.01):
+    """Write the free-T descriptor of the device MPC update to an MPC file (include/omg_b200.h:
+    omg_mpc_freet_read)."""
+    _write_mpc(mpc_freeT_desc(problem, update_time, sample_time), MPC_FREET_FIELDS, path)
 
 
 class B200Solver(object):
