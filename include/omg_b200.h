@@ -224,7 +224,9 @@ int omg_feas_batch_host(omg_problem* h, int32_t B,
  * in place).  offs/lens/ncols: HOST int arrays [n_blocks]; T: HOST array of the
  * n_blocks row-major matrices, concatenated.  Asynchronous on `stream`; the block
  * descriptor is uploaded on the first call and whenever it changes (the host arrays are
- * copied before the call returns). */
+ * copied before the call returns).  The x row is staged in shared memory: 8 n bytes, opted in
+ * above 48 KB, up to 227 KB.  Rejected with a message: null pointers, n_blocks < 0, a block with
+ * len < 1 or ncol < 1 or outside x (off < 0 or off + len * ncol > n), and n above 227 KB of x row. */
 int omg_shift_batch(omg_problem* h, int32_t B, double* x,
                     int32_t n_blocks, const int32_t* offs, const int32_t* lens,
                     const int32_t* ncols, const double* T, void* stream);
@@ -260,7 +262,10 @@ int omg_last_timing(omg_problem* h, float* kernel_ms, int32_t* launches);
  * S_blk [nsamp x len] (precomputed basis / derivative rows) to every column:
  * out[b] = concat_blk( [col][sample] ), DEVICE x [B][n] and out [B][sum nsamp*ncols].
  * Asynchronous on `stream`; descriptor and S are uploaded on the first call of the host
- * thread and whenever they change (copied before the call returns). */
+ * thread and whenever they change (copied before the call returns).  The x row is staged in
+ * shared memory as by omg_shift_batch (8 n bytes, up to 227 KB).  Rejected with a message: null
+ * pointers, n_blocks < 0, a block with len < 1, ncol < 1 or nsamp < 1 or outside x, and n above
+ * 227 KB of x row. */
 int omg_sample_batch(int32_t B, int32_t n, const double* x, int32_t n_blocks,
                      const int32_t* offs, const int32_t* lens, const int32_t* ncols,
                      const int32_t* nsamp, const double* S, double* out, void* stream);

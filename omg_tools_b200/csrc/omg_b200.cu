@@ -2866,17 +2866,46 @@ static int desc_upload(DescCache& c, int device, const std::vector<int>& iv, con
   return 0;
 }
 
+// Blocks of omg_shift_batch / omg_sample_batch (nsamp: NULL for the shift) and the x row both
+// kernels hold in shared memory: false with a message naming `fn` when a block is empty or outside
+// x, when the matrices or outputs (*n_mat, *n_out entries) outgrow the kernels' int offsets, or when
+// the x row exceeds the shared memory of a block.  Above 48 KB the kernel `kfn` is opted in.
+static bool fixed_desc(const std::string& fn, int32_t n, int32_t n_blocks, const int32_t* offs, const int32_t* lens,
+                       const int32_t* ncols, const int32_t* nsamp, const void* kfn, int64_t* n_mat, int64_t* n_out) {
+  *n_mat = 0; *n_out = 0;
+  for (int k = 0; k < n_blocks; ++k) {
+    const std::string blk = fn + ": block " + std::to_string(k) + ": ";
+    if (lens[k] < 1) { set_err(blk + "basis length " + std::to_string(lens[k]) + " < 1"); return false; }
+    if (nsamp && nsamp[k] < 1) { set_err(blk + "nsamp " + std::to_string(nsamp[k]) + " < 1"); return false; }
+    if (ncols[k] < 1 || offs[k] < 0 || (int64_t)offs[k] + (int64_t)lens[k] * ncols[k] > n) {
+      set_err(blk + "columns outside x"); return false; }
+    *n_mat += (int64_t)(nsamp ? nsamp[k] : lens[k]) * lens[k];
+    *n_out += (int64_t)(nsamp ? nsamp[k] : lens[k]) * ncols[k];
+  }
+  if (*n_mat > INT32_MAX || *n_out > INT32_MAX) { set_err(fn + ": matrices or output beyond 2^31 entries"); return false; }
+  const size_t smem = sizeof(double) * (size_t)std::max<int32_t>(n, 0);
+  if (smem > 227 * 1024) { set_err(fn + ": x row exceeds the shared memory of a block"); return false; }
+  if (smem > 48 * 1024 &&
+      cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
+    set_err(fn + ": cudaFuncSetAttribute failed: " + cudaGetErrorString(cudaGetLastError())); return false; }
+  return true;
+}
+
 int omg_shift_batch(omg_problem* h, int32_t B, double* x, int32_t n_blocks, const int32_t* offs,
                     const int32_t* lens, const int32_t* ncols, const double* Tm, void* stream_) {
-  if (!h || !x || !offs || !lens || !ncols || !Tm) { set_err("null argument"); return -1; }
-  if (B <= 0 || n_blocks <= 0) return 0;
-  cudaStream_t stream = (cudaStream_t)stream_;
+  const std::string f("omg_shift_batch");
+  if (!h || !x || !offs || !lens || !ncols || !Tm) { set_err(f + ": null argument"); return -1; }
+  if (n_blocks < 0) { set_err(f + ": n_blocks " + std::to_string(n_blocks) + " < 0"); return -1; }
   CK(cudaSetDevice(h->device));
+  int64_t tot = 0, n_out = 0;
+  if (!fixed_desc(f, h->T.n, n_blocks, offs, lens, ncols, nullptr, (const void*)omg_shift_kernel, &tot, &n_out))
+    return -1;
+  if (B <= 0 || n_blocks == 0) return 0;
+  cudaStream_t stream = (cudaStream_t)stream_;
   std::vector<int> iv(4 * (size_t)n_blocks);
-  int tot = 0;
-  for (int b = 0; b < n_blocks; ++b) {
-    iv[b] = offs[b]; iv[n_blocks + b] = lens[b]; iv[2 * n_blocks + b] = ncols[b]; iv[3 * n_blocks + b] = tot;
-    tot += lens[b] * lens[b];
+  for (int b = 0, t = 0; b < n_blocks; ++b) {
+    iv[b] = offs[b]; iv[n_blocks + b] = lens[b]; iv[2 * n_blocks + b] = ncols[b]; iv[3 * n_blocks + b] = t;
+    t += lens[b] * lens[b];
   }
   if (!h->shift_desc) h->shift_desc = new DescCache();
   DescCache& c = *h->shift_desc;
@@ -2890,15 +2919,18 @@ int omg_shift_batch(omg_problem* h, int32_t B, double* x, int32_t n_blocks, cons
 int omg_sample_batch(int32_t B, int32_t n, const double* x, int32_t n_blocks, const int32_t* offs,
                      const int32_t* lens, const int32_t* ncols, const int32_t* nsamp,
                      const double* Sm, double* out, void* stream_) {
-  if (!x || !offs || !lens || !ncols || !nsamp || !Sm || !out) { set_err("null argument"); return -1; }
-  if (B <= 0 || n_blocks <= 0) return 0;
+  const std::string f("omg_sample_batch");
+  if (!x || !offs || !lens || !ncols || !nsamp || !Sm || !out) { set_err(f + ": null argument"); return -1; }
+  if (n_blocks < 0) { set_err(f + ": n_blocks " + std::to_string(n_blocks) + " < 0"); return -1; }
+  int64_t stot = 0, otot = 0;
+  if (!fixed_desc(f, n, n_blocks, offs, lens, ncols, nsamp, (const void*)omg_sample_kernel, &stot, &otot)) return -1;
+  if (B <= 0 || n_blocks == 0) return 0;
   cudaStream_t stream = (cudaStream_t)stream_;
   std::vector<int> iv(6 * (size_t)n_blocks);
-  int stot = 0, otot = 0;
-  for (int b = 0; b < n_blocks; ++b) {
+  for (int b = 0, s = 0, o = 0; b < n_blocks; ++b) {
     iv[b] = offs[b]; iv[n_blocks + b] = lens[b]; iv[2 * n_blocks + b] = ncols[b]; iv[3 * n_blocks + b] = nsamp[b];
-    iv[4 * n_blocks + b] = stot; stot += nsamp[b] * lens[b];
-    iv[5 * n_blocks + b] = otot; otot += nsamp[b] * ncols[b];
+    iv[4 * n_blocks + b] = s; s += nsamp[b] * lens[b];
+    iv[5 * n_blocks + b] = o; o += nsamp[b] * ncols[b];
   }
   int device = 0;
   CK(cudaGetDevice(&device));

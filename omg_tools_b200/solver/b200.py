@@ -728,14 +728,20 @@ class B200Solver(object):
 
     def shift_batch_device(self, X, blocks, stream=None):
         """In-place warm-start shift of spline variables (torch CUDA tensor X
-        [B, n]); blocks = [(offset, len_basis, n_columns, T)]."""
-        import torch
+        [B, n]); blocks = [(offset, len_basis, n_columns, T)], T of shape
+        len_basis x len_basis."""
         offs = np.array([b[0] for b in blocks], dtype=np.int32)
         lens = np.array([b[1] for b in blocks], dtype=np.int32)
         ncols = np.array([b[2] for b in blocks], dtype=np.int32)
+        for b in blocks:
+            if np.shape(b[3]) != (b[1], b[1]):
+                raise ValueError('a block of length %d needs a %d x %d T, got %s'
+                                 % (b[1], b[1], b[1], np.shape(b[3])))
         Tm = np.concatenate([np.asarray(b[3], dtype=np.float64).reshape(-1)
                              for b in blocks])
         on_gpu = _check_device_tensors((X,), self.lib)
+        if X.dim() != 2 or X.shape[1] != self.n:
+            raise ValueError('X must be [B, n]')
         self._check(self.lib.omg_shift_batch(
             self._handle, X.shape[0], X.data_ptr(), len(blocks), offs.ctypes.data,
             lens.ctypes.data, ncols.ctypes.data, Tm.ctypes.data,
@@ -866,6 +872,12 @@ def sample_batch(X, blocks, stream=None):
     offs = np.array([b[0] for b in blocks], dtype=np.int32)
     lens = np.array([b[1] for b in blocks], dtype=np.int32)
     ncols = np.array([b[2] for b in blocks], dtype=np.int32)
+    for b in blocks:
+        if np.ndim(b[3]) != 2 or np.shape(b[3])[1] != b[1]:
+            raise ValueError('a block of length %d needs an S with %d columns, got shape %s'
+                             % (b[1], b[1], np.shape(b[3])))
+    if X.dim() != 2:
+        raise ValueError('X must be [B, n]')
     nsamp = np.array([np.asarray(b[3]).shape[0] for b in blocks], dtype=np.int32)
     Sm = np.concatenate([np.ascontiguousarray(b[3], dtype=np.float64).reshape(-1) for b in blocks])
     out = torch.empty((X.shape[0], int((nsamp * ncols).sum())), dtype=torch.float64, device=X.device)

@@ -45,9 +45,12 @@ extern double omg_emu_smem[];      // the running block's dynamic shared memory
 
 #define OMG_DYN_SHARED(name) static double* const name = omg_emu_smem
 #define OMG_LAUNCH(kern, grid, block, smem, stream, ...) \
-  omg_emu_launch((grid), (block), (size_t)(smem), [&]() { kern(__VA_ARGS__); })
+  omg_emu_launch((const void*)(kern), (grid), (block), (size_t)(smem), [&]() { kern(__VA_ARGS__); })
 
-void omg_emu_launch(int grid, int block, size_t smem_bytes, const std::function<void()>& body);
+// As on the device, a launch with more than 48 KB of dynamic shared memory fails (the kernel does
+// not run, cudaGetLastError reports it) unless cudaFuncSetAttribute(kern,
+// cudaFuncAttributeMaxDynamicSharedMemorySize, >= smem) was called for that kernel.
+void omg_emu_launch(const void* kern, int grid, int block, size_t smem_bytes, const std::function<void()>& body);
 void __syncthreads();
 static inline void __threadfence() {}
 double __shfl_down_sync(unsigned mask, double v, int delta);
@@ -64,7 +67,7 @@ static inline int max(int a, int b) { return a > b ? a : b; }
 
 // ---- runtime API subset used by the host side of omg_b200.cu ----------------------
 typedef int cudaError_t;
-enum { cudaSuccess = 0, cudaErrorEmu = 1 };
+enum { cudaSuccess = 0, cudaErrorEmu = 1, cudaErrorInvalidValue = 2 };
 typedef void* cudaStream_t;
 typedef struct omg_emu_event { double t; }* cudaEvent_t;
 enum cudaMemcpyKind { cudaMemcpyHostToDevice, cudaMemcpyDeviceToHost, cudaMemcpyDeviceToDevice, cudaMemcpyDefault };
@@ -88,7 +91,7 @@ static inline cudaError_t cudaGetDeviceProperties(cudaDeviceProp* p, int) {
   p->multiProcessorCount = 2; p->sharedMemPerBlockOptin = 232448; p->sharedMemPerMultiprocessor = 233472;
   return cudaSuccess; }
 static inline cudaError_t cudaFuncGetAttributes(cudaFuncAttributes* a, const void*) { a->sharedSizeBytes = 1024; a->numRegs = 0; return cudaSuccess; }
-static inline cudaError_t cudaFuncSetAttribute(const void*, cudaFuncAttribute, int) { return cudaSuccess; }
+cudaError_t cudaFuncSetAttribute(const void* kern, cudaFuncAttribute, int value);
 static inline cudaError_t cudaOccupancyMaxActiveBlocksPerMultiprocessor(int* occ, const void*, int nt, size_t smem) {
   int o = (int)((233472 - 1024) / (smem + 1024)); const int by_threads = 2048 / (nt > 0 ? nt : 1);
   if (o > by_threads) o = by_threads; *occ = o; return cudaSuccess; }
@@ -99,5 +102,6 @@ cudaError_t cudaEventElapsedTime(float* ms, cudaEvent_t a, cudaEvent_t b);
 cudaError_t cudaEventDestroy(cudaEvent_t e);
 static inline cudaError_t cudaStreamSynchronize(cudaStream_t) { return cudaSuccess; }
 static inline cudaError_t cudaDeviceSynchronize() { return cudaSuccess; }
-static inline cudaError_t cudaGetLastError() { return cudaSuccess; }
-static inline const char* cudaGetErrorString(cudaError_t e) { return e == cudaSuccess ? "no error" : "emulation error"; }
+cudaError_t cudaGetLastError();
+static inline const char* cudaGetErrorString(cudaError_t e) {
+  return e == cudaSuccess ? "no error" : e == cudaErrorInvalidValue ? "invalid argument" : "emulation error"; }

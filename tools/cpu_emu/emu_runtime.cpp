@@ -6,6 +6,7 @@
 #include <stdio.h>
 #include <sys/mman.h>
 #include <time.h>
+#include <map>
 #include <vector>
 
 uint3 threadIdx, blockIdx;
@@ -48,6 +49,9 @@ int cur = 0, n_threads = 0, alive = 0, arrived = 0;
 int warp_alive[kMaxThreads / 32], warp_arrived[kMaxThreads / 32];
 double shfl_slot[kMaxThreads];
 const std::function<void()>* body = nullptr;
+std::map<const void*, int> max_dyn_smem;     // cudaFuncAttributeMaxDynamicSharedMemorySize per kernel
+cudaError_t last_error = cudaSuccess;
+const size_t kDefaultDynSmem = 48 * 1024, kOptinDynSmem = 232448;   // H100: 48 KB default, 227 KB opt-in
 
 void yield_to_scheduler() { omg_emu_switch(&fibers[cur].sp, sched_sp); }
 
@@ -117,9 +121,21 @@ long long clock64() {
   return (long long)ts.tv_sec * 1000000000LL + ts.tv_nsec;
 }
 
-void omg_emu_launch(int grid, int block, size_t smem_bytes, const std::function<void()>& fn) {
-  if (block <= 0 || block > kMaxThreads || (block & 31) || smem_bytes > sizeof(omg_emu_smem)) {
+cudaError_t cudaFuncSetAttribute(const void* kern, cudaFuncAttribute, int value) {
+  if (value < 0 || (size_t)value > kOptinDynSmem) return last_error = cudaErrorInvalidValue;
+  max_dyn_smem[kern] = value;
+  return cudaSuccess;
+}
+
+cudaError_t cudaGetLastError() { const cudaError_t e = last_error; last_error = cudaSuccess; return e; }
+
+void omg_emu_launch(const void* kern, int grid, int block, size_t smem_bytes, const std::function<void()>& fn) {
+  if (block <= 0 || block > kMaxThreads || (block & 31)) {
     fprintf(stderr, "omg_emu_launch: unsupported launch (block %d, smem %zu)\n", block, smem_bytes); abort(); }
+  if (smem_bytes > kDefaultDynSmem) {
+    const auto it = max_dyn_smem.find(kern);
+    if (it == max_dyn_smem.end() || (size_t)it->second < smem_bytes) { last_error = cudaErrorInvalidValue; return; }
+  }
   if (!stacks) {
     stacks = static_cast<char*>(mmap(nullptr, kStack * kMaxThreads, PROT_READ | PROT_WRITE,
                                      MAP_PRIVATE | MAP_ANONYMOUS | MAP_NORESERVE, -1, 0));
