@@ -526,7 +526,8 @@ void omg_tables_free(omg_tables* tables);
  *            every shift block is multiplied by its T matrix (omg_shift_batch).  P[b] is
  *            p_template with state0, input0, poseT = stateT[b], t = t_rel, T = horizon and the
  *            obstacles' x, v, a (and theta) written in.
- *   solve    omg_solve_batch with the problem's own bounds, shared by all instances.
+ *   solve    omg_solve_batch with the problem's own bounds, shared by all instances (with obstacles
+ *            attached: each instance's own bound row, see omg_mpc_attach_obstacles).
  *   commit   status 0: the x row takes the solution, t_prev_b = t_b, state_traj[b] and
  *            input_traj[b] receive the plan's values and derivatives / horizon at
  *            t_rel + k * sample_time (k < trajectory_length; a sample past the horizon reads 0),
@@ -536,9 +537,11 @@ void omg_tables_free(omg_tables* tables);
  *            (Point2Point::update returns false).  status[b] and iters[b] are always written.
  * Obstacles are supplied on every call in their current state (the reference's obstacle_t):
  * obstacles[b] holds n_obs records of 3 * n_dim + 1 doubles, {x, v, a, theta}; theta is read only
- * for a rotating obstacle.  A free motion time (FreeTPoint2point) has its own descriptor and create
- * call below and shares every other call.  Not covered: several vehicles, other vehicles, run-time
- * bounds (updateBounds), predict_shift and provide_prediction. */
+ * for a rotating obstacle.  The rest of obstacle_t, each obstacle's shape (checkpoints and radii) and
+ * its avoid flag (updateBounds), is per-instance state set by omg_mpc_set_obstacles after
+ * omg_mpc_attach_obstacles (below).  A free motion time (FreeTPoint2point) has its own descriptor and
+ * create call below and shares every other call.  Not covered: several vehicles, other vehicles,
+ * time-based constraint shutdown, predict_shift and provide_prediction. */
 typedef struct omg_mpc omg_mpc;   /* opaque handle */
 
 typedef struct omg_mpc_desc {
@@ -666,6 +669,52 @@ int omg_mpc_time(omg_mpc* mpc, double* t_out);
 /* The warm start and parameter rows handed to the last solve, DEVICE x0_out [B][n] and p_out
  * [B][n_par] (either may be NULL).  Asynchronous on `stream`. */
 int omg_mpc_last_problem(omg_mpc* mpc, double* x0_out, double* p_out, void* stream);
+
+/* ---- obstacle shapes and avoidance (the rest of the reference's obstacle_t) ------------------
+ * Point2Point::update() takes, per obstacle, its checkpoints and radii, written into the parameters
+ * on every call (export.py _create_fillParameterDict), and an avoid flag: when it is false,
+ * updateBounds sets the bounds of that obstacle's own constraint rows to -inf / +inf for the solve
+ * (export.py _create_updateBounds; Point2Point.cpp:213-218).  The hyperplane rows of the
+ * environment and the vehicle's own rows are not among them.  Here both are per-instance state of a
+ * handle of either kind: once attached, every update writes instance b's stored shapes into P[b]
+ * after the template (and the obstacles' x, v, a, theta) and solves with instance b's own bound row.
+ *
+ * The descriptor lists the obstacles in environment order (the order of omg_mpc_desc's obs_off). */
+typedef struct omg_mpc_obstacles_desc {
+  int32_t n_obs;
+  const int32_t* chk_off;         /* [n_obs] offset in p of the checkpoints x0, y0, x1, y1, ... */
+  const int32_t* chk_len;         /* [n_obs] n_chk * n_dim */
+  const int32_t* rad_off;         /* [n_obs] offset in p of the radii */
+  const int32_t* rad_len;         /* [n_obs] n_chk */
+  const int32_t* row_off;         /* [n_obs] first g row of the obstacle's own constraints */
+  const int32_t* row_len;         /* [n_obs] their number */
+} omg_mpc_obstacles_desc;
+
+/* Obstacle files: the container of omg_mpc_read under the magic "OMGOBS\0\0", records named after
+ * the fields of omg_mpc_obstacles_desc (written by omg_tools_b200.solver.b200.save_mpc_obstacles).
+ * Returns a heap object (release it with omg_mpc_obstacles_release) or NULL (omg_last_error). */
+omg_mpc_obstacles_desc* omg_mpc_obstacles_read(const char* path);
+void omg_mpc_obstacles_release(omg_mpc_obstacles_desc* desc);
+
+/* Allocate and initialise the handle's per-instance obstacle state: every shape is the template's
+ * (p_template at chk_off / rad_off), every avoid flag is set, and each instance's bound row [m] is
+ * the tables' bounds.  Synchronous; call it once, before updates that are captured in a graph.
+ * Returns -1 with a message for: a null argument, an n_obs that differs from the handle's, p entries
+ * outside p, a checkpoint length other than n_dim times the radius length (which must be >= 1),
+ * row ranges outside [0, m) or overlapping, a row in a range whose table bounds are an equality
+ * (the equality rows are part of the solver's symbolic analysis), and a handle that already has
+ * obstacles attached. */
+int omg_mpc_attach_obstacles(omg_mpc* mpc, const omg_mpc_obstacles_desc* desc);
+
+/* Set the obstacles' shapes and avoid flags of every instance until the next set call (updates and
+ * omg_mpc_recover leave them as they are).  DEVICE buffers: shapes [B][sum_k (n_dim + 1) n_chk_k],
+ * per obstacle its checkpoints (chk_len doubles) and then its radii (rad_len), the field order of
+ * obstacle_t; avoid [B][n_obs], nonzero: avoid.  Either may be NULL, which keeps that part.
+ * Asynchronous on `stream` and capturable in a CUDA graph.  Returns -1 when no obstacles are
+ * attached. */
+int omg_mpc_set_obstacles(omg_mpc* mpc, const double* shapes, const int32_t* avoid, void* stream);
+/* Same call with HOST buffers (synchronous). */
+int omg_mpc_set_obstacles_host(omg_mpc* mpc, const double* shapes, const int32_t* avoid);
 
 const char* omg_last_error(void);
 int omg_abi_version(void);

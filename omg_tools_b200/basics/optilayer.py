@@ -532,15 +532,20 @@ class OptiChild(object):
 
     @classmethod
     def _make_label(cls, label):
-        """vehicle -> vehicle0, vehicle1, ... (reference optilayer.py:538-550)."""
+        """vehicle -> vehicle0, vehicle1, ... (reference optilayer.py:538-550): the label with the first
+        index from its own (0 without one) that no child has taken yet.  The reference finds it by one
+        recursive call per taken index; this loop gives the same labels without tying the number of
+        children a process may create to the recursion limit."""
         parts = [''.join(g) for _, g in groupby(label, str.isalpha)]
         index, rest = parts[-1], ''.join(parts[:-1])
-        if index.isdigit():
-            if label in cls._labels:
-                return cls._make_label(rest + str(int(index) + 1))
-            cls._labels.append(label)
-            return label
-        return cls._make_label(label + str(0))
+        if not index.isdigit():
+            label, index, rest = label + '0', '0', label
+        k = int(index)
+        while label in cls._labels:
+            k += 1
+            label = rest + str(k)
+        cls._labels.append(label)
+        return label
 
     # ---------------------------------------------------------------------
     # definition of symbols, variables, parameters, constraints, objective

@@ -3434,12 +3434,41 @@ struct MpcDev {
   int* ns;                  // [B] integrate: the samples of U the next prediction spans
   int* rows;                // [B] the rows solved by this update, ascending
   int* n_rows;              // [1]
+  // obstacle shapes and avoidance (omg_mpc_attach_obstacles); shapes == nullptr: not attached
+  int m, n_shape;           // g rows; doubles of one instance's shape record
+  const int* obs_geo;       // [n_obs][6]: chk_off, chk_len, rad_off, rad_len, row_off, row_len
+  double* shapes;           // [B][n_shape] per obstacle its checkpoints, then its radii
+  double* lbg;              // [B][m] each instance's bounds
+  double* ubg;              // [B][m]
 };
 
 enum { OMG_MPC_COLD = 0, OMG_MPC_ACCEPTED = 1, OMG_MPC_FAILED = 2 };
 
 // numpy.round(x, 6)
 __device__ __forceinline__ double omg_round6(double x) { return rint(x * 1e6) / 1e6; }
+
+// The obstacles of instance b into its parameter row pb, after the template copy (one thread): their
+// x, v, a (and theta) from obs[b] and, with obstacles attached, their stored checkpoints and radii.
+__device__ void omg_mpc_write_obstacles(const MpcDev& M, int b, const double* __restrict__ obs, double* pb) {
+  const int nd = M.nd, rl = 3 * nd + 1;
+  for (int k = 0; k < M.n_obs; ++k) {
+    const double* o = obs + ((size_t)b * M.n_obs + k) * rl;
+    const int* off = M.obs_off + 4 * k;
+    for (int c = 0; c < nd; ++c) {
+      pb[off[0] + c] = o[c];
+      pb[off[1] + c] = o[nd + c];
+      pb[off[2] + c] = o[2 * nd + c];
+    }
+    if (M.obs_kind[k]) pb[off[3]] = o[3 * nd];
+  }
+  if (!M.shapes) return;
+  const double* s = M.shapes + (size_t)b * M.n_shape;
+  for (int k = 0; k < M.n_obs; ++k) {
+    const int* g = M.obs_geo + 6 * k;
+    for (int i = 0; i < g[1]; ++i) pb[g[0] + i] = *s++;
+    for (int i = 0; i < g[3]; ++i) pb[g[2] + i] = *s++;
+  }
+}
 
 // Shared memory: source x row [n] | warm start [n].
 __global__ void omg_mpc_prepare_kernel(const MpcDev M, const double* __restrict__ state0,
@@ -3493,17 +3522,7 @@ __global__ void omg_mpc_prepare_kernel(const MpcDev M, const double* __restrict_
   }
   pb[M.p_t] = fmod(omg_round6(tb), kt);
   pb[M.p_T] = M.horizon;
-  const int rl = 3 * nd + 1;
-  for (int k = 0; k < M.n_obs; ++k) {
-    const double* o = obs + ((size_t)b * M.n_obs + k) * rl;
-    const int* off = M.obs_off + 4 * k;
-    for (int c = 0; c < nd; ++c) {
-      pb[off[0] + c] = o[c];
-      pb[off[1] + c] = o[nd + c];
-      pb[off[2] + c] = o[2 * nd + c];
-    }
-    if (M.obs_kind[k]) pb[off[3]] = o[3 * nd];
-  }
+  omg_mpc_write_obstacles(M, b, obs, pb);
   M.rec[b] = 0;
 }
 
@@ -3643,17 +3662,7 @@ __global__ void omg_mpc_prepare_free_kernel(const MpcDev M, const double* __rest
     pb[M.p_input0 + c] = u0[c];
     pb[M.p_poseT + c] = stT[c];
   }
-  const int rl = 3 * nd + 1;
-  for (int k = 0; k < M.n_obs; ++k) {
-    const double* o = obs + ((size_t)b * M.n_obs + k) * rl;
-    const int* off = M.obs_off + 4 * k;
-    for (int c = 0; c < nd; ++c) {
-      pb[off[0] + c] = o[c];
-      pb[off[1] + c] = o[nd + c];
-      pb[off[2] + c] = o[2 * nd + c];
-    }
-    if (M.obs_kind[k]) pb[off[3]] = o[3 * nd];
-  }
+  omg_mpc_write_obstacles(M, b, obs, pb);
 }
 
 // The rows that are not stopped, in ascending order, and their count: one block, a scan per chunk
@@ -3756,6 +3765,28 @@ __global__ void omg_mpc_flag_kernel(int B, const int* __restrict__ mask, int* __
   if (b < B && mask[b]) rec[b] = 1;
 }
 
+// One instance per block: store its shape record and rewrite the rows of its obstacles in its bound
+// row, the tables' bounds lbg / ubg where avoid is set and -inf / +inf where it is not (updateBounds).
+__global__ void omg_mpc_set_obstacles_kernel(const MpcDev M, const double* __restrict__ shapes,
+                                             const int* __restrict__ avoid, const double* __restrict__ lbg,
+                                             const double* __restrict__ ubg) {
+  const int b = blockIdx.x, t = threadIdx.x, nt = blockDim.x;
+  if (b >= M.B) return;
+  if (shapes)
+    for (int i = t; i < M.n_shape; i += nt) M.shapes[(size_t)b * M.n_shape + i] = shapes[(size_t)b * M.n_shape + i];
+  if (!avoid) return;
+  double* lb = M.lbg + (size_t)b * M.m;
+  double* ub = M.ubg + (size_t)b * M.m;
+  for (int k = 0; k < M.n_obs; ++k) {
+    const int* g = M.obs_geo + 6 * k;
+    const bool on = avoid[(size_t)b * M.n_obs + k] != 0;
+    for (int r = g[4] + t; r < g[4] + g[5]; r += nt) {
+      lb[r] = on ? lbg[r] : -INFINITY;
+      ub[r] = on ? ubg[r] : INFINITY;
+    }
+  }
+}
+
 #define OMG_MPC_NT 128
 
 struct omg_mpc {
@@ -3769,6 +3800,8 @@ struct omg_mpc {
   // device staging of omg_mpc_update_host
   double *s0 = nullptr, *sT = nullptr, *obs = nullptr, *xtraj = nullptr, *utraj = nullptr;
   int *st = nullptr, *it = nullptr;
+  // device staging of omg_mpc_set_obstacles_host (allocated by omg_mpc_attach_obstacles)
+  double* hshapes = nullptr; int* havoid = nullptr;
 };
 
 namespace {
@@ -3794,27 +3827,33 @@ const MpcField kMpcFreeTFields[] = {
   MF(x_template, 3), MF(p_template, 3),
 };
 #undef MF
+#define MF(f, k) {#f, k, offsetof(omg_mpc_obstacles_desc, f)}
+const MpcField kMpcObstacleFields[] = {
+  MF(n_obs, 0), MF(chk_off, 2), MF(chk_len, 2), MF(rad_off, 2), MF(rad_len, 2), MF(row_off, 2), MF(row_len, 2),
+};
+#undef MF
 template <class D> struct OwnedDesc { D desc; std::vector<void*> blocks; };
 
-// An MPC file of the fields `fields` into a heap descriptor; a record that is not one of them but one
-// of `other` (no) marks the other kind of MPC file, which `other_reader` reads.
+// A file of the record container with magic `magic` (`what`: its name in messages) of the fields
+// `fields` into a heap descriptor; a record that is not one of them but one of `other` (no) marks the
+// other kind of MPC file, which `other_reader` reads.
 template <class D>
 D* mpc_read_file(const char* path, const MpcField* fields, int nf, const MpcField* other, int no,
-                 const char* other_reader) {
+                 const char* other_reader, const char* magic_ = "OMGMPC\0\0", const std::string& what = "MPC") {
   FILE* fp = path ? fopen(path, "rb") : nullptr;
-  if (!fp) { set_err(std::string("cannot open MPC file ") + (path ? path : "(null)")); return nullptr; }
+  if (!fp) { set_err("cannot open " + what + " file " + (path ? path : "(null)")); return nullptr; }
   OwnedDesc<D>* O = new OwnedDesc<D>();
   memset(&O->desc, 0, sizeof(O->desc));
   bool ok = true;
   char magic[8]; int32_t ver = 0, nrec = 0;
-  if (fread(magic, 1, 8, fp) != 8 || memcmp(magic, "OMGMPC\0\0", 8) != 0) { set_err("not an omg MPC file"); ok = false; }
-  if (ok && (fread(&ver, 4, 1, fp) != 1 || fread(&nrec, 4, 1, fp) != 1)) { set_err("truncated MPC file"); ok = false; }
-  if (ok && ver != OMG_ABI_VERSION) { set_err("MPC file written for another ABI version"); ok = false; }
+  if (fread(magic, 1, 8, fp) != 8 || memcmp(magic, magic_, 8) != 0) { set_err("not an omg " + what + " file"); ok = false; }
+  if (ok && (fread(&ver, 4, 1, fp) != 1 || fread(&nrec, 4, 1, fp) != 1)) { set_err("truncated " + what + " file"); ok = false; }
+  if (ok && ver != OMG_ABI_VERSION) { set_err(what + " file written for another ABI version"); ok = false; }
   std::vector<char> seen(nf, 0);
   for (int r = 0; ok && r < nrec; ++r) {
     char name[24]; int32_t dtype = 0, pad = 0; int64_t count = 0;
     if (fread(name, 1, 24, fp) != 24 || fread(&dtype, 4, 1, fp) != 1 || fread(&pad, 4, 1, fp) != 1 ||
-        fread(&count, 8, 1, fp) != 1 || count < 0) { set_err("truncated MPC file"); ok = false; break; }
+        fread(&count, 8, 1, fp) != 1 || count < 0) { set_err("truncated " + what + " file"); ok = false; break; }
     name[23] = 0;
     int k = -1;
     for (int q = 0; q < nf; ++q) if (strcmp(fields[q].name, name) == 0) { k = q; break; }
@@ -3823,7 +3862,7 @@ D* mpc_read_file(const char* path, const MpcField* fields, int nf, const MpcFiel
     if (other_kind) {
       set_err(std::string("this MPC file is of the other kind: read it with ") + other_reader); ok = false; break; }
     const int kind = k < 0 ? -1 : fields[k].kind;
-    if (k < 0 || dtype != (kind == 1 || kind == 3 ? 1 : 0)) { set_err(std::string("unknown record in MPC file: ") + name); ok = false; break; }
+    if (k < 0 || dtype != (kind == 1 || kind == 3 ? 1 : 0)) { set_err("unknown record in " + what + " file: " + name); ok = false; break; }
     const size_t esz = dtype ? 8 : 4;
     char* base = reinterpret_cast<char*>(&O->desc) + fields[k].off;
     if (kind < 2) {
@@ -3831,14 +3870,14 @@ D* mpc_read_file(const char* path, const MpcField* fields, int nf, const MpcFiel
     } else {
       void* blk = malloc((size_t)(count > 0 ? count : 1) * esz);
       O->blocks.push_back(blk);
-      if (!blk || (count > 0 && fread(blk, esz, (size_t)count, fp) != (size_t)count)) { set_err("truncated MPC file"); ok = false; break; }
+      if (!blk || (count > 0 && fread(blk, esz, (size_t)count, fp) != (size_t)count)) { set_err("truncated " + what + " file"); ok = false; break; }
       *reinterpret_cast<void**>(base) = blk;
     }
     seen[k] = 1;
   }
   fclose(fp);
   for (int q = 0; ok && q < nf; ++q)
-    if (!seen[q]) { set_err(std::string("MPC file lacks ") + fields[q].name); ok = false; }
+    if (!seen[q]) { set_err(what + " file lacks " + fields[q].name); ok = false; }
   if (!ok) { for (void* b : O->blocks) free(b); delete O; return nullptr; }
   return &O->desc;
 }
@@ -4094,12 +4133,17 @@ int omg_mpc_update(omg_mpc* q, const double* state0, const double* stateT, const
   omg_problem* h = q->h;
   CK(cudaSetDevice(h->device));
   const int B = q->M.B;
+  // the tables' bounds, shared by every instance, or with obstacles attached each instance's own row
+  const bool own = q->M.shapes != nullptr;
+  const double* lbg = own ? q->M.lbg : h->lbg;
+  const double* ubg = own ? q->M.ubg : h->ubg;
+  const int32_t shared = own ? 0 : 1;
   if (q->free_T) {
     OMG_LAUNCH(omg_mpc_prepare_free_kernel, B, OMG_MPC_NT, q->smem_prepare, stream, q->M, state0, stateT, obstacles);
     CK(cudaGetLastError());
     OMG_LAUNCH(omg_mpc_rows_kernel, 1, 256, 256 * sizeof(int), stream, B, q->M.stop, q->M.rows, q->M.n_rows);
     CK(cudaGetLastError());
-    if (solve_batch_rows(h, B, q->M.X0, q->M.P, h->lbg, h->ubg, 1, nullptr, q->M.Xn, q->lam, q->f, status, iters,
+    if (solve_batch_rows(h, B, q->M.X0, q->M.P, lbg, ubg, shared, nullptr, q->M.Xn, q->lam, q->f, status, iters,
                          q->M.rows, q->M.n_rows, stream))
       return -1;
     OMG_LAUNCH(omg_mpc_commit_free_kernel, B, OMG_MPC_NT, q->smem_commit, stream, q->M, status, iters, state_traj,
@@ -4109,7 +4153,7 @@ int omg_mpc_update(omg_mpc* q, const double* state0, const double* stateT, const
   }
   OMG_LAUNCH(omg_mpc_prepare_kernel, B, OMG_MPC_NT, q->smem_prepare, stream, q->M, state0, stateT, obstacles);
   CK(cudaGetLastError());
-  if (omg_solve_batch(h, B, q->M.X0, q->M.P, h->lbg, h->ubg, 1, nullptr, q->M.Xn, q->lam, q->f, status, iters, stream))
+  if (omg_solve_batch(h, B, q->M.X0, q->M.P, lbg, ubg, shared, nullptr, q->M.Xn, q->lam, q->f, status, iters, stream))
     return -1;
   OMG_LAUNCH(omg_mpc_commit_kernel, B, OMG_MPC_NT, q->smem_commit, stream, q->M, status, state_traj, input_traj);
   CK(cudaGetLastError());
@@ -4174,6 +4218,97 @@ int omg_mpc_last_problem(omg_mpc* q, double* x0_out, double* p_out, void* stream
   const size_t b = q->M.B;
   if (x0_out) CK(cudaMemcpyAsync(x0_out, q->M.X0, b * q->M.n * 8, cudaMemcpyDeviceToDevice, stream));
   if (p_out) CK(cudaMemcpyAsync(p_out, q->M.P, b * q->M.n_par * 8, cudaMemcpyDeviceToDevice, stream));
+  return 0;
+}
+
+omg_mpc_obstacles_desc* omg_mpc_obstacles_read(const char* path) {
+  const int nf = (int)(sizeof(kMpcObstacleFields) / sizeof(kMpcObstacleFields[0]));
+  return mpc_read_file<omg_mpc_obstacles_desc>(path, kMpcObstacleFields, nf, nullptr, 0, "", "OMGOBS\0\0", "obstacle");
+}
+
+void omg_mpc_obstacles_release(omg_mpc_obstacles_desc* desc) { mpc_free_file(desc); }
+
+int omg_mpc_attach_obstacles(omg_mpc* q, const omg_mpc_obstacles_desc* D) {
+  const std::string f("omg_mpc_attach_obstacles: ");
+  if (!q || !D) { set_err(f + "null argument"); return -1; }
+  MpcDev& M = q->M;
+  if (M.shapes) { set_err(f + "this handle already has obstacles attached"); return -1; }
+  if (D->n_obs != M.n_obs) {
+    set_err(f + "the descriptor has " + std::to_string(D->n_obs) + " obstacles, the handle " + std::to_string(M.n_obs));
+    return -1;
+  }
+  const int n_obs = M.n_obs, m = q->h->T.m, np_ = M.n_par;
+  if (n_obs > 0 && (!D->chk_off || !D->chk_len || !D->rad_off || !D->rad_len || !D->row_off || !D->row_len)) {
+    set_err(f + "null descriptor array"); return -1; }
+  CK(cudaSetDevice(q->h->device));
+  std::vector<double> lbg(m), ubg(m), ptpl(np_);
+  CK(cudaMemcpy(lbg.data(), q->h->lbg, (size_t)m * 8, cudaMemcpyDeviceToHost));
+  CK(cudaMemcpy(ubg.data(), q->h->ubg, (size_t)m * 8, cudaMemcpyDeviceToHost));
+  CK(cudaMemcpy(ptpl.data(), M.p_tpl, (size_t)np_ * 8, cudaMemcpyDeviceToHost));
+  std::vector<int> geo(6 * (size_t)n_obs);
+  std::vector<char> taken(m, 0);
+  std::vector<double> rec;                 // one instance's shape record: the template's shapes
+  for (int k = 0; k < n_obs; ++k) {
+    const std::string o = "obstacle " + std::to_string(k) + " ";
+    if (!mpc_range(f, o + "checkpoints", D->chk_off[k], D->chk_len[k], np_) ||
+        !mpc_range(f, o + "radii", D->rad_off[k], D->rad_len[k], np_) ||
+        !mpc_range(f, o + "rows", D->row_off[k], D->row_len[k], m)) return -1;
+    if (D->rad_len[k] < 1 || D->chk_len[k] != M.nd * D->rad_len[k]) {
+      set_err(f + o + "has " + std::to_string(D->chk_len[k]) + " checkpoint coordinates and " +
+              std::to_string(D->rad_len[k]) + " radii; n_dim = " + std::to_string(M.nd) + " coordinates per radius");
+      return -1;
+    }
+    for (int r = D->row_off[k]; r < D->row_off[k] + D->row_len[k]; ++r) {
+      if (taken[r]) { set_err(f + o + "rows overlap another obstacle's at row " + std::to_string(r)); return -1; }
+      if (lbg[r] == ubg[r]) {
+        set_err(f + o + "row " + std::to_string(r) + " is an equality; its bounds cannot be freed"); return -1; }
+      taken[r] = 1;
+    }
+    const int g[6] = {D->chk_off[k], D->chk_len[k], D->rad_off[k], D->rad_len[k], D->row_off[k], D->row_len[k]};
+    std::copy(g, g + 6, geo.begin() + 6 * k);
+    rec.insert(rec.end(), ptpl.begin() + g[0], ptpl.begin() + g[0] + g[1]);
+    rec.insert(rec.end(), ptpl.begin() + g[2], ptpl.begin() + g[2] + g[3]);
+  }
+  const size_t B = M.B, ns = rec.size();
+  std::vector<double> shapes(B * ns), lb(B * m), ub(B * m);
+  for (size_t b = 0; b < B; ++b) {
+    std::copy(rec.begin(), rec.end(), shapes.begin() + b * ns);
+    std::copy(lbg.begin(), lbg.end(), lb.begin() + b * m);
+    std::copy(ubg.begin(), ubg.end(), ub.begin() + b * m);
+  }
+  bool ok = true;
+  const int* d_geo = (const int*)mpc_alloc(q, 4 * geo.size(), geo.data(), &ok);
+  double* d_shapes = (double*)mpc_alloc(q, 8 * shapes.size(), shapes.data(), &ok);
+  double* d_lbg = (double*)mpc_alloc(q, 8 * lb.size(), lb.data(), &ok);
+  double* d_ubg = (double*)mpc_alloc(q, 8 * ub.size(), ub.data(), &ok);
+  q->hshapes = (double*)mpc_alloc(q, 8 * shapes.size(), nullptr, &ok);
+  q->havoid = (int*)mpc_alloc(q, 4 * B * n_obs, nullptr, &ok);
+  if (!ok) { set_err(f + "device allocation/upload failed"); return -1; }
+  M.m = m; M.n_shape = (int)ns; M.obs_geo = d_geo; M.lbg = d_lbg; M.ubg = d_ubg;
+  M.shapes = d_shapes;                     // (last: a non-null shapes marks the handle attached)
+  return 0;
+}
+
+int omg_mpc_set_obstacles(omg_mpc* q, const double* shapes, const int32_t* avoid, void* stream_) {
+  if (!q) { set_err("omg_mpc_set_obstacles: null argument"); return -1; }
+  if (!q->M.shapes) { set_err("omg_mpc_set_obstacles: no obstacles attached (omg_mpc_attach_obstacles)"); return -1; }
+  if (!shapes && !avoid) return 0;
+  CK(cudaSetDevice(q->h->device));
+  OMG_LAUNCH(omg_mpc_set_obstacles_kernel, q->M.B, OMG_MPC_NT, 0, (cudaStream_t)stream_, q->M, shapes, avoid,
+             q->h->lbg, q->h->ubg);
+  CK(cudaGetLastError());
+  return 0;
+}
+
+int omg_mpc_set_obstacles_host(omg_mpc* q, const double* shapes, const int32_t* avoid) {
+  if (!q) { set_err("omg_mpc_set_obstacles_host: null argument"); return -1; }
+  if (!q->M.shapes) { set_err("omg_mpc_set_obstacles_host: no obstacles attached (omg_mpc_attach_obstacles)"); return -1; }
+  CK(cudaSetDevice(q->h->device));
+  const size_t b = q->M.B;
+  if (shapes) CK(cudaMemcpy(q->hshapes, shapes, b * q->M.n_shape * 8, cudaMemcpyHostToDevice));
+  if (avoid) CK(cudaMemcpy(q->havoid, avoid, b * q->M.n_obs * 4, cudaMemcpyHostToDevice));
+  if (omg_mpc_set_obstacles(q, shapes ? q->hshapes : nullptr, avoid ? q->havoid : nullptr, nullptr)) return -1;
+  CK(cudaStreamSynchronize(nullptr));
   return 0;
 }
 

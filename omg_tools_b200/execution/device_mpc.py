@@ -17,6 +17,11 @@ from the plan's own T, the prediction and the trajectory samples are taken on th
 axis, and an instance whose plan is shorter than update_time, or that has arrived at its goal, stops:
 it is not solved again (status MPC_STOPPED = -1, 0 iterations) until recover().  motion_time() gives
 each instance's T, and so how much of the returned trajectory is plan.
+
+The rest of the reference's obstacle_t, each obstacle's shape (checkpoints and radii) and its avoid
+flag, is per-instance state that set_obstacles() changes (include/omg_b200.h,
+omg_mpc_set_obstacles): an obstacle that is not avoided has its own constraint rows freed for that
+instance's solves, as the reference's updateBounds does.
 """
 import ctypes as C
 
@@ -64,6 +69,7 @@ class DeviceMPC(object):
         if not self._handle:
             raise RuntimeError('%s failed: %s' % (create, self.lib.omg_last_error().decode()))
         self.n, self.n_par = desc['n'], desc['n_par']
+        self._problem, self._obs_desc, self._attached = problem, None, False
         f64 = dict(dtype=torch.float64, device=self.dev)
         i32 = dict(dtype=torch.int32, device=self.dev)
         shape = (self.B, self.trajectory_length, self.n_dim)
@@ -92,6 +98,53 @@ class DeviceMPC(object):
             self.input_traj.data_ptr(), self.status.data_ptr(), self.iters.data_ptr(),
             b200._stream_handle(on_gpu, state0.device, stream)))
         return self.state_traj, self.input_traj, self.status, self.iters
+
+    def _obstacles(self):
+        if self._obs_desc is None:
+            self._obs_desc = b200.mpc_obstacles_desc(self._problem)
+        return self._obs_desc
+
+    @property
+    def shape_layout(self):
+        """The record set_obstacles takes per instance: a list with, per obstacle, the slices of its
+        checkpoints (x0, y0, x1, y1, ... : n_chk * n_dim values) and of its radii (n_chk values), and
+        the record's length."""
+        d, out, o = self._obstacles(), [], 0
+        for k in range(self.n_obs):
+            nc, nr = int(d['chk_len'][k]), int(d['rad_len'][k])
+            out.append((slice(o, o + nc), slice(o + nc, o + nc + nr)))
+            o += nc + nr
+        return out, o
+
+    def set_obstacles(self, shapes=None, avoid=None, stream=None):
+        """Set the obstacles' shapes and avoid flags of every instance for this and the following
+        updates, until the next call (recover() does not change them).  shapes: float64 device tensor
+        [B, record length of shape_layout], per obstacle its checkpoints and then its radii; avoid:
+        int32 device tensor [B, n_obs], nonzero to avoid the obstacle.  None keeps that part.  Before
+        the first call every shape is the problem's own and every obstacle is avoided.
+
+        The first call attaches the obstacle state to the handle, which allocates and synchronises
+        the device; every later call is stream-ordered and can be captured in a CUDA graph."""
+        B, n_shape = self.B, self.shape_layout[1]
+        if shapes is not None:
+            b200._check_device_tensors((shapes,), self.lib)
+            if tuple(shapes.shape) != (B, n_shape):
+                raise ValueError('shapes must be [B, %d] = [%d, %d]' % (n_shape, B, n_shape))
+        if avoid is not None:
+            b200._check_int_tensors((avoid,))
+            if tuple(avoid.shape) != (B, self.n_obs):
+                raise ValueError('avoid must be [B, n_obs] = [%d, %d]' % (B, self.n_obs))
+        ref = shapes if shapes is not None else avoid
+        if not self._attached:
+            D, keep = b200.pack_mpc_obstacles_desc(self._obstacles())
+            self._check(self.lib.omg_mpc_attach_obstacles(self._handle, C.byref(D)))
+            del keep
+            self._attached = True
+        if ref is None:
+            return
+        self._check(self.lib.omg_mpc_set_obstacles(
+            self._handle, None if shapes is None else shapes.data_ptr(), None if avoid is None else avoid.data_ptr(),
+            b200._stream_handle(ref.is_cuda, ref.device, stream)))
 
     def recover(self, mask):
         """Cold-start the instances with mask[b] true on their next update (Point2Point::recover)."""

@@ -105,6 +105,15 @@ class _MpcFreeTDesc(C.Structure):
     _fields_ = [(name, _CTYPE[kind]) for name, kind in MPC_FREET_FIELDS]
 
 
+# include/omg_b200.h omg_mpc_obstacles_desc, in the same notation
+MPC_OBSTACLE_FIELDS = [('n_obs', 'i'), ('chk_off', 'I'), ('chk_len', 'I'), ('rad_off', 'I'), ('rad_len', 'I'),
+                       ('row_off', 'I'), ('row_len', 'I')]
+
+
+class _MpcObstaclesDesc(C.Structure):
+    _fields_ = [(name, _CTYPE[kind]) for name, kind in MPC_OBSTACLE_FIELDS]
+
+
 MPC_PREDICTION = {'ideal': 0, 'integrate': 1}
 MPC_STOPPED = -1        # status of an instance that was not solved because it has stopped
 
@@ -120,7 +129,8 @@ EXPORTS = ['omg_abi_version', 'omg_last_error', 'omg_default_options',
            'omg_mpc_read', 'omg_mpc_free_desc', 'omg_mpc_create', 'omg_mpc_destroy', 'omg_mpc_update',
            'omg_mpc_update_host', 'omg_mpc_recover', 'omg_mpc_time', 'omg_mpc_last_problem',
            'omg_mpc_freet_read', 'omg_mpc_freet_release', 'omg_mpc_create_freet', 'omg_mpc_motion_time',
-           'omg_solve_batch_rows']
+           'omg_solve_batch_rows', 'omg_mpc_obstacles_read', 'omg_mpc_obstacles_release',
+           'omg_mpc_attach_obstacles', 'omg_mpc_set_obstacles', 'omg_mpc_set_obstacles_host']
 
 _lib = None
 
@@ -211,6 +221,13 @@ def bind(lib):
     lib.omg_mpc_create_freet.argtypes = [vp, C.POINTER(_MpcFreeTDesc), C.c_int32, C.c_int32, C.c_int32]
     lib.omg_mpc_create_freet.restype = C.c_void_p
     lib.omg_mpc_motion_time.argtypes = [vp] * 3
+    lib.omg_mpc_obstacles_read.argtypes = [C.c_char_p]
+    lib.omg_mpc_obstacles_read.restype = C.POINTER(_MpcObstaclesDesc)
+    lib.omg_mpc_obstacles_release.argtypes = [C.POINTER(_MpcObstaclesDesc)]
+    lib.omg_mpc_obstacles_release.restype = None
+    lib.omg_mpc_attach_obstacles.argtypes = [vp, C.POINTER(_MpcObstaclesDesc)]
+    lib.omg_mpc_set_obstacles.argtypes = [vp] * 4
+    lib.omg_mpc_set_obstacles_host.argtypes = [vp] * 3
     lib.omg_solve_batch_rows.argtypes = [vp, C.c_int32, vp, vp, vp, vp, C.c_int32, vp] + [vp] * 8
     lib.omg_tables_read.argtypes = [C.c_char_p]
     lib.omg_tables_read.restype = C.POINTER(_Tables)
@@ -482,6 +499,30 @@ def mpc_freeT_desc(problem, update_time=0.1, sample_time=0.01):
     return desc
 
 
+def mpc_obstacles_desc(problem):
+    """The obstacle descriptor of the device MPC update (include/omg_b200.h, omg_mpc_obstacles_desc)
+    of a problem mpc_desc or mpc_freeT_desc describes, as a dict of the MPC_OBSTACLE_FIELDS: per
+    obstacle, in environment order, the p entries of its checkpoints and radii and the g rows of its
+    own constraints, the rows the reference's updateBounds frees when the obstacle is not avoided
+    (export.py _create_updateBounds).  Raises NotImplementedError as those do."""
+    _, par, _, desc = _mpc_vehicle(problem)
+    father = problem.father
+    cons = father._con_struct.entries
+    out = {k: [] for k, _ in MPC_OBSTACLE_FIELDS[1:]}
+    for o in problem.environment.obstacles:
+        chk, rad = par[(o.label, 'checkpoints')], par[(o.label, 'rad')]
+        rows = [cons[(None, o._add_label(name))][:2] for name in o._constraints]
+        lo = rows[0][0] if rows else 0
+        if any(r[0] != lo + sum(q[1] for q in rows[:i]) for i, r in enumerate(rows)):
+            raise NotImplementedError('the constraint rows of obstacle %s are not one contiguous run' % o.label)
+        for key, v in (('chk_off', chk[0]), ('chk_len', chk[1]), ('rad_off', rad[0]), ('rad_len', rad[1]),
+                       ('row_off', lo), ('row_len', sum(r[1] for r in rows))):
+            out[key].append(v)
+    out = {k: np.array(v, dtype=np.int32) for k, v in out.items()}
+    out['n_obs'] = desc['n_obs']
+    return out
+
+
 def _pack(desc, fields, cls):
     keep, D = _Keep(), cls()
     for name, kind in fields:
@@ -496,15 +537,20 @@ def pack_mpc_desc(desc):
     return _pack(desc, MPC_FIELDS, _MpcDesc)
 
 
+def pack_mpc_obstacles_desc(desc):
+    """mpc_obstacles_desc dict -> (ctypes omg_mpc_obstacles_desc, keep-alive object)."""
+    return _pack(desc, MPC_OBSTACLE_FIELDS, _MpcObstaclesDesc)
+
+
 def pack_mpc_freeT_desc(desc):
     """mpc_freeT_desc dict -> (ctypes omg_mpc_freeT_desc, keep-alive object)."""
     return _pack(desc, MPC_FREET_FIELDS, _MpcFreeTDesc)
 
 
-def _write_mpc(desc, fields, path):
+def _write_mpc(desc, fields, path, magic=b'OMGMPC\0\0'):
     import struct
     with open(path, 'wb') as fp:
-        fp.write(b'OMGMPC\0\0')
+        fp.write(magic)
         fp.write(struct.pack('<ii', ABI_VERSION, len(fields)))
         for name, kind in fields:
             dtype = 1 if kind in 'dD' else 0
@@ -524,6 +570,12 @@ def save_mpc_freeT(problem, path, update_time=0.1, sample_time=0.01):
     """Write the free-T descriptor of the device MPC update to an MPC file (include/omg_b200.h:
     omg_mpc_freet_read)."""
     _write_mpc(mpc_freeT_desc(problem, update_time, sample_time), MPC_FREET_FIELDS, path)
+
+
+def save_mpc_obstacles(problem, path):
+    """Write the obstacle descriptor of the device MPC update to an obstacle file (include/omg_b200.h:
+    omg_mpc_obstacles_read), for native callers of omg_mpc_attach_obstacles."""
+    _write_mpc(mpc_obstacles_desc(problem), MPC_OBSTACLE_FIELDS, path, b'OMGOBS\0\0')
 
 
 class B200Solver(object):
